@@ -78,6 +78,7 @@ def load_library():
         "bani_ctx_set_flag": (C.c_int, [vp, C.c_char_p, i64]),
         "bani_ctx_profile_enable": (C.c_int, [vp, C.c_int]),
         "bani_ctx_profile_read": (C.c_int, [vp, vp, vp, vp, vp, i32, P(i32)]),
+        "bani_ctx_path_counts": (C.c_int, [vp, vp, vp, i32, P(i32)]),
         "bani_host_alloc": (C.c_int, [C.c_size_t, P(vp)]),
         "bani_host_free": (None, [vp]),
         "bani_genome_create": (C.c_int, [vp, i32, vp, vp, P(vp)]),
@@ -120,7 +121,7 @@ def load_library():
 EXPORTED_SYMBOLS = [
     "bani_last_error", "bani_version", "bani_params_default", "bani_recommended_window_size", "bani_device_count",
     "bani_stat_min_hits_relaxed", "bani_stat_identity", "bani_ctx_create", "bani_ctx_destroy", "bani_ctx_params",
-    "bani_ctx_sync", "bani_ctx_stream", "bani_ctx_launch_count", "bani_ctx_set_flag", "bani_ctx_profile_enable", "bani_ctx_profile_read", "bani_host_alloc", "bani_host_free", "bani_genome_create",
+    "bani_ctx_sync", "bani_ctx_stream", "bani_ctx_launch_count", "bani_ctx_set_flag", "bani_ctx_profile_enable", "bani_ctx_profile_read", "bani_ctx_path_counts", "bani_host_alloc", "bani_host_free", "bani_genome_create",
     "bani_genome_create_batch", "bani_pack_contig", "bani_genome_create_packed_batch", "bani_genome_destroy", "bani_genome_info", "bani_genome_decode", "bani_index_build",
     "bani_index_destroy", "bani_index_stats", "bani_index_minimizers", "bani_index_save", "bani_index_load", "bani_index_contigs",
     "bani_qsketch_from_index", "bani_index_lookup", "bani_map_genome",
@@ -201,8 +202,17 @@ class Context:
         return int(self.lib.bani_ctx_launch_count(self.h))
 
     def set_flag(self, name, value):
-        """bani_ctx_set_flag: "sketch_reuse", "max_hits_per_piece", "frag_l1_max", "l2e_buckets"."""
+        """bani_ctx_set_flag: "sketch_reuse", "max_hits_per_piece", "frag_l1_max", "l2e_buckets", "l2_stage",
+        "upload_group_words", "frags_per_piece", "event_bytes_per_piece", "cgi_table_queries", "l2_fast", "count_paths"."""
         _check(self.lib.bani_ctx_set_flag(self.h, name.encode(), int(value)))
+
+    def path_counts(self):
+        """{branch: count} of the mapping path since the last read (bani_ctx_path_counts; needs count_paths = 1)."""
+        nmax = 64
+        names = (C.c_char * 32 * nmax)()
+        cnt = (C.c_uint64 * nmax)(); n = C.c_int32()
+        _check(self.lib.bani_ctx_path_counts(self.h, names, cnt, nmax, C.byref(n)))
+        return {names[i].value.decode(): int(cnt[i]) for i in range(n.value)}
 
     def profile(self, on=True):
         _check(self.lib.bani_ctx_profile_enable(self.h, 1 if on else 0))

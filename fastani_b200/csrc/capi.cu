@@ -1,5 +1,6 @@
 // capi.cu -- the extern "C" boundary declared in include/fastani_b200.h
 #include "common.cuh"
+#include <algorithm>
 #include <cstring>
 #include <cstdlib>
 
@@ -11,6 +12,13 @@ struct bani_qsketch { bani::QSketch *qs; };
 namespace bani {
 static thread_local std::string g_err;
 void set_last_error(const std::string &m) { g_err = m; }
+const char *const PATH_NAMES[NPATH] = {
+  "l1.class0", "l1.class1", "l1.class2", "l1.class3", "l1.class4", "l1.class5", "l1.class6", "l1.class7", "l1.class8",
+  "l1.class9", "l1.class10", "l1.class11", "l1.class12", "l1.device_wide",
+  "lookup.walk_saturated", "lookup.walk_full_bucket",
+  "l2.events_nt64", "l2.events_nt128", "l2.events_nt256", "l2.dir1024", "l2.dir4096", "l2.staged", "l2.direct",
+  "l2.exact_at_bounds", "l2.exact_total",
+  "piece.mapped", "piece.split_hits", "piece.split_events", "cgi.passes"};
 }
 
 using namespace bani;
@@ -149,7 +157,24 @@ int bani_ctx_set_flag(bani_ctx *ctx, const char *name, int64_t value)
   else if (n == "l2e_buckets") { if (value != 0 && value != 1024 && value != 4096) fail(BANI_ERR_ARG, "l2e_buckets must be 0, 1024 or 4096"); f.l2eBuckets = (int)value; }
   else if (n == "l2_stage") f.l2Stage = value != 0;
   else if (n == "upload_group_words") { if (value < 1) fail(BANI_ERR_ARG, "upload_group_words must be positive"); f.uploadGroupWords = value; }
+  else if (n == "frags_per_piece") { if (value < 1 || value > (1ll << 18)) fail(BANI_ERR_ARG, "frags_per_piece must be in [1, 2^18]"); f.fragsPerPiece = value; }
+  else if (n == "event_bytes_per_piece") { if (value < 0) fail(BANI_ERR_ARG, "event_bytes_per_piece must not be negative"); f.eventBytesPerPiece = value; }
+  else if (n == "cgi_table_queries") { if (value < 0) fail(BANI_ERR_ARG, "cgi_table_queries must not be negative"); f.cgiTableQueries = value; }
+  else if (n == "l2_fast") f.l2Fast = value != 0;
+  else if (n == "count_paths") f.countPaths = value != 0;
   else fail(BANI_ERR_ARG, "unknown flag '%s'", name);
+  return BANI_OK;
+  BANI_CATCH
+}
+
+int bani_ctx_path_counts(bani_ctx *ctx, char (*names)[32], uint64_t *counts, int32_t n_max, int32_t *n)
+{
+  BANI_TRY
+  if (!ctx || !n || (n_max > 0 && (!names || !counts))) fail(BANI_ERR_ARG, "null argument");
+  const int cnt = std::min<int>(n_max, NPATH);
+  for (int i = 0; i < cnt; i++) { strncpy(names[i], PATH_NAMES[i], 31); names[i][31] = 0; counts[i] = ctx->c.paths[i]; }
+  for (int i = 0; i < NPATH; i++) ctx->c.paths[i] = 0;
+  *n = cnt;
   return BANI_OK;
   BANI_CATCH
 }

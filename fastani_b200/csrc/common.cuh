@@ -208,7 +208,28 @@ struct CtxFlags {
                                               //    (more instructions for about half the DRAM traffic: the faster choice on H100, DESIGN.md
                                               //    section 6); 0: direct stores for every candidate, kept as a tested alternative
   long long uploadGroupWords = 16ll << 20;    // packed words (16 bases each) per upload group of the host-packed ingest
+  // Test switches that bring branches of the mapping path, which otherwise need very large inputs, down to small ones.
+  // Results never depend on them.
+  long long fragsPerPiece = 1ll << 18;        // fragments per query piece (map.cu: FRAG_MAX is the default and the maximum)
+  long long eventBytesPerPiece = 0;           // a piece whose L2 event streams take more is halved; 0 = a quarter of device memory
+  long long cgiTableQueries = 0;              // queries per pass of the identity reduction; 0 = as many as 3 GiB of bin table hold
+  int l2Fast = 1;                             // 0: every L2 candidate goes to the exact kernel (l2_kernel)
+  int countPaths = 0;                         // 1: count which branch of the mapping path ran (bani_ctx_path_counts)
 };
+
+// Branches of the mapping path, counted when CtxFlags::countPaths is set (names: capi.cu, bani_ctx_path_counts).  What a
+// counter counts: fragments per L1 size class; probes that walked the sorted keys; L2 candidates with window events per
+// event-kernel variant; candidates left to the exact kernel after the bounds pass and in total; pieces and passes.
+// The per-piece counters (everything but piece.split_*) are those of the pieces that were mapped, not of those split.
+enum PathId {
+  P_L1_CLASS0 = 0, P_L1_DEVICE_WIDE = 13,                    // 13 == FRAG_NCLASS
+  P_LOOKUP_WALK_SATURATED, P_LOOKUP_WALK_FULL_BUCKET,
+  P_L2_EVENTS_NT64, P_L2_EVENTS_NT128, P_L2_EVENTS_NT256, P_L2_DIR1024, P_L2_DIR4096, P_L2_STAGED, P_L2_DIRECT,
+  P_L2_EXACT_AT_BOUNDS, P_L2_EXACT_TOTAL,
+  P_PIECE_MAPPED, P_PIECE_SPLIT_HITS, P_PIECE_SPLIT_EVENTS, P_CGI_PASSES,
+  NPATH
+};
+extern const char *const PATH_NAMES[NPATH];
 
 struct Ctx {
   int device = 0;
@@ -233,6 +254,7 @@ struct Ctx {
     traceT = t;
   }
   uint64_t launches = 0;             // kernels of this library launched so far (CUB's not counted)
+  uint64_t paths[NPATH] = {};        // branch counters since the last bani_ctx_path_counts (flags.countPaths)
   bool profiling = false;
   struct ProfEv { const char *name; cudaEvent_t a, b; double bytes; };
   std::vector<ProfEv> profEvents;
@@ -322,6 +344,7 @@ void qsketch_map(Ctx *ctx, const Index *ix, const QSketch *const *sketches, int3
 // hits.cu : per-fragment gather + shared-memory sort + L1 candidate regions
 static constexpr unsigned long long FRAG_L1_MAX = 8192;   // hits per fragment handled inside one CTA
 static constexpr int FRAG_NCLASS = 13;                    // size classes: 256 * {1,2,3,4,5,6,7,8,10,12,16,24,32} hits
+static_assert(P_L1_DEVICE_WIDE == FRAG_NCLASS, "one path counter per L1 size class");
 __host__ __device__ inline int frag_class_items(int cls)
 {
   return cls < 8 ? cls + 1 : (cls == 8 ? 10 : cls == 9 ? 12 : cls == 10 ? 16 : cls == 11 ? 24 : 32);

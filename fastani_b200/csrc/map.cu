@@ -140,9 +140,11 @@ __device__ __forceinline__ int seg_of(const uint32_t *segStart, int F, uint32_t 
 // Thread per query hash.  One 32-byte sector of the probe table answers almost every probe (hit or miss): bucket = low
 // bits of the hash, 4 entries {x = (hash & ~0xFF) | min(count, 255), y = offset}.  Only a full bucket without a match, or a
 // saturated count, walks the sorted keys (bucket directory over the top bits, then a short binary search).
+// walkCtr (null unless the context counts paths): probes that walked for a saturated count [0] / a full bucket [1].
 __global__ void lookup_kernel(const uint32_t *fragHash, uint32_t T, const uint2 *tab, uint32_t tabMask,
                               const uint32_t *ukeys, const uint32_t *uoff, const uint32_t *dir, int dirBits,
-                              const uint32_t *filt, uint32_t filtMask, uint32_t *hitLo, uint32_t *hitCnt)
+                              const uint32_t *filt, uint32_t filtMask, uint32_t *hitLo, uint32_t *hitCnt,
+                              unsigned long long *walkCtr)
 {
   const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t > T) return;
@@ -162,6 +164,7 @@ __global__ void lookup_kernel(const uint32_t *fragHash, uint32_t T, const uint2 
     else if ((ex[sl] & 0xFFFFFF00u) == key) { found = true; cnt = ex[sl] & 0xFFu; lo0 = ey[sl]; }
   }
   if ((found && cnt == 255u) || (!found && full)) {
+    if (walkCtr) atomicAdd(&walkCtr[found ? 0 : 1], 1ull);
     cnt = 0; lo0 = 0;
     const uint32_t b = h >> (32 - dirBits);
     uint32_t lo = dir[b], hi = dir[b + 1];
@@ -980,8 +983,9 @@ __global__ void compact_sketch_kernel(const uint32_t *raw, const uint32_t *rawSt
 }
 
 // fragments per piece: the working set of a piece (hit staging, L2 event streams: ~25 GB for 2^18 fragments of config 3)
-// must fit an 80 GB device next to the index of a 1000-genome shard (~32 GB)
+// must fit an 80 GB device next to the index of a 1000-genome shard (~32 GB).  The switch frags_per_piece lowers it.
 static constexpr uint64_t FRAG_MAX = 1u << 18;
+static uint64_t frags_per_piece(const Ctx *ctx) { return std::min<uint64_t>(FRAG_MAX, (uint64_t)std::max(1ll, ctx->flags.fragsPerPiece)); }
 
 // A query as the sketch stage sees it: a contig-length table plus either the packed bases (stage A) or the first contig
 // ordinal inside the hint index (stage A': the genome is a member of the index, its bases are not needed).
@@ -1036,6 +1040,7 @@ static QSketch *qsketch_build(Ctx *ctx, const std::vector<QuerySrc> &srcs, const
   qs->queryId.resize(nq); qs->totalFragments.assign(nq, 0);
   for (int i = 0; i < nq; i++) qs->queryId[i] = queryIds ? queryIds[i] : i;
 
+  const uint64_t fragMax = frags_per_piece(ctx);
   int q0 = 0;
   while (q0 < nq) {
     // ---- fragment sources of this piece (Map::mapQuery, computeMap.hpp:131-189)
@@ -1049,7 +1054,7 @@ static QSketch *qsketch_build(Ctx *ctx, const std::vector<QuerySrc> &srcs, const
       const Genome *Q = qsrc.G;
       uint64_t nf = 0;
       for (int c = 0; c < qsrc.nContigs; c++) { int L = qsrc.len[c]; if (!(L < w || L < k || L < fragLen)) nf += L / fragLen; }
-      if (q1 > q0 && (uint64_t)F64 + nf > FRAG_MAX) break;
+      if (q1 > q0 && (uint64_t)F64 + nf > fragMax) break;
       const int32_t mem = hint ? qsrc.member : -1;
       if (mem < 0 && !Q) fail(BANI_ERR_INTERNAL, "query without bases and without an index to derive it from");
       if (mem < 0) Q->wait_ready(st);                                  // its bases are hashed: the upload must have landed
@@ -1319,10 +1324,11 @@ QSketch *qsketch_merge(Ctx *ctx, const QSketch *const *sketches, int32_t n)
     out->totalFragments.insert(out->totalFragments.end(), qs->totalFragments.begin(), qs->totalFragments.end());
     for (const auto &pc : qs->pieces) srcs.push_back(Src{pc.get(), qBase + pc->q0});
   }
+  const uint64_t fragMax = frags_per_piece(ctx);
   size_t i = 0;
   while (i < srcs.size()) {
     size_t j = i; uint64_t F = 0, T = 0;
-    while (j < srcs.size() && (j == i || (F + (uint64_t)srcs[j].pc->F <= FRAG_MAX && T + srcs[j].pc->T < 0xfffffff0ull &&
+    while (j < srcs.size() && (j == i || (F + (uint64_t)srcs[j].pc->F <= fragMax && T + srcs[j].pc->T < 0xfffffff0ull &&
                                           srcs[j].qBase == srcs[j - 1].qBase + srcs[j - 1].pc->nq))) { F += (uint64_t)srcs[j].pc->F; T += srcs[j].pc->T; j++; }
     auto pc = std::make_unique<QPiece>();
     pc->q0 = srcs[i].qBase; pc->F = (int32_t)F; pc->T = T;
@@ -1383,6 +1389,15 @@ static std::unique_ptr<QPiece> slice_piece(Ctx *ctx, const QPiece &pc, int qa, i
   return sl;
 }
 
+// path counter (flags.countPaths only): candidates the exact kernel l2_kernel will solve (cBest == -1)
+static uint64_t count_exact(Ctx *ctx, const int32_t *d_cBest, uint32_t C)
+{
+  std::vector<int32_t> h(C);
+  BANI_CUDA(cudaMemcpyAsync(h.data(), d_cBest, 4 * (size_t)C, cudaMemcpyDeviceToHost, ctx->stream));
+  BANI_CUDA(cudaStreamSynchronize(ctx->stream));
+  return (uint64_t)std::count(h.begin(), h.end(), -1);
+}
+
 // ------------------------------------------------------------------ host orchestration of stages C..H
 void map_queries(Ctx *ctx, const Index *ix, const Genome *const *queries, int32_t nq,
                  bool wantRows, bool wantCgi, MapOutput &out)
@@ -1414,6 +1429,10 @@ void qsketch_map(Ctx *ctx, const Index *ix, const QSketch *const *sketches, int3
   // the 2-way table holds a bounded number of queries at a time
   uint64_t qMaxByTable = 1u << 30;
   if (wantCgi && ix->totalBins) qMaxByTable = std::max<uint64_t>(1, ((uint64_t)3 << 30) / (4 * ix->totalBins));
+  if (ctx->flags.cgiTableQueries > 0) qMaxByTable = std::min<uint64_t>(qMaxByTable, (uint64_t)ctx->flags.cgiTableQueries);
+  // a piece whose L2 event streams would take more is mapped in halves
+  const double evLimit = ctx->flags.eventBytesPerPiece > 0 ? (double)ctx->flags.eventBytesPerPiece : 0.25 * (double)ctx->memTotal;
+  const bool countPaths = ctx->flags.countPaths != 0;
 
   DevBuf<uint32_t> table; DevBuf<uint8_t> touched; DevBuf<int32_t> d_gce;
   uint64_t tableQ = 0;
@@ -1439,8 +1458,10 @@ void qsketch_map(Ctx *ctx, const Index *ix, const QSketch *const *sketches, int3
     const uint64_t T = pc.T;
     const int smax = pc.smax;
     bool split = false;
+    uint64_t pp[NPATH] = {};                 // path counters of this piece, kept if it is not split
     // halve the piece at a query boundary (by fragments) and do the halves instead
-    auto split_in_halves = [&]() {
+    auto split_in_halves = [&](PathId why) {
+      if (countPaths) ctx->paths[why]++;
       int qm = 1;
       while (qm < nQc - 1 && pc.qFragOff[qm] < F / 2) qm++;
       slices.push_back(slice_piece(ctx, pc, qm, nQc)); work.push_front(slices.back().get());
@@ -1465,21 +1486,24 @@ void qsketch_map(Ctx *ctx, const Index *ix, const QSketch *const *sketches, int3
         BANI_SCRATCH(uint32_t, hitLo, T + 1);
         BANI_SCRATCH(uint32_t, hitCnt, T + 1);
         BANI_SCRATCH(unsigned long long, hitOff, T + 1);
+        DevBuf<unsigned long long> walkCtr;
+        if (countPaths) { walkCtr.alloc(2, st); BANI_CUDA(cudaMemsetAsync(walkCtr.p, 0, 16, st)); }
         { Stage sg(ctx, "lookup", 12.0 * T);
           // the membership filter pays when most probes miss: not for queries that are genomes of this very index
           const bool useFilt = ix->filt.p && pc.memberOf != ix->uid;
           lookup_kernel<<<nblk(T + 1), 256, 0, st>>>(fragHash.p, (uint32_t)T, ix->tab.p, (1u << ix->tabBits) - 1u, ix->ukeys.p, ix->uoff.p,
                                                    ix->dir.p, ix->dirBits, useFilt ? ix->filt.p : nullptr,
-                                                   useFilt ? (uint32_t)((1ull << ix->filtBits) - 1ull) : 0u, hitLo.p, hitCnt.p);
+                                                   useFilt ? (uint32_t)((1ull << ix->filtBits) - 1ull) : 0u, hitLo.p, hitCnt.p, walkCtr.p);
           ctx->launches++;
           size_t tb = cub_scan_u64_temp(T + 1);
           BANI_SCRATCH(uint8_t, tmp, tb);
           cub_exclusive_sum_u32_to_u64(tmp.p, tb, hitCnt.p, (uint64_t *)hitOff.p, T + 1, st); }
         unsigned long long N = 0;
         BANI_CUDA(cudaMemcpyAsync(&N, hitOff.p + T, 8, cudaMemcpyDeviceToHost, st));
+        if (countPaths) BANI_CUDA(cudaMemcpyAsync(pp + P_LOOKUP_WALK_SATURATED, walkCtr.p, 16, cudaMemcpyDeviceToHost, st));
         BANI_CUDA(cudaStreamSynchronize(st));
         ctx->mark("piece: lookup done");
-        if (N > maxHits && nQc > 1) split_in_halves();          // too many hits for one pass
+        if (N > maxHits && nQc > 1) split_in_halves(P_PIECE_SPLIT_HITS);          // too many hits for one pass
         if (!split && N > 0xfffffff0ull) fail(BANI_ERR_LIMIT, "one query genome gathers more than 2^32 index hits");
         if (!split) out.ctr.hits += N;
 
@@ -1501,6 +1525,7 @@ void qsketch_map(Ctx *ctx, const Index *ix, const QSketch *const *sketches, int3
             frag_classify(ctx, segStart.p, hitOff.p, F, candCount.p, fragClass.p, classCount.p, classList.p, (unsigned long long)maxFast);
             BANI_CUDA(cudaMemcpyAsync(hClass, classCount.p, sizeof hClass, cudaMemcpyDeviceToHost, st));
             BANI_CUDA(cudaStreamSynchronize(st));
+            for (int i = 0; i <= FRAG_NCLASS; i++) pp[P_L1_CLASS0 + i] += hClass[i];
             FragL1Args fa; fa.segStart = segStart.p; fa.sCount = sCount.p; fa.F = F; fa.hitLo = hitLo.p; fa.hitCnt = hitCnt.p; fa.hitOff = hitOff.p;
             fa.posIdx = ix->posIdx.p; fa.recPos = ix->pos8.p; fa.minHits = ctx->d_minHits.p; fa.fragLen = fragLen;
             fa.keyBits = 1; while (fa.keyBits < 32 && (1ull << fa.keyBits) < ix->M) fa.keyBits++;
@@ -1591,7 +1616,8 @@ void qsketch_map(Ctx *ctx, const Index *ix, const QSketch *const *sketches, int3
               lp.rec8 = ix->rec8.p; lp.recLink = ix->link.p; lp.blkMax = ix->blkMax.p; lp.stage = ctx->flags.l2Stage;
               // fast path: needs the window links of the index (cmw >= 2) and ranks that fit the event code
               // (and whose per-warp state fits the shared-memory budget of l2_seq_kernel: larger sketches take l2_kernel)
-              lp.sLimit = (cmw >= 2 && ix->cmw == cmw && ix->rec8.p) ? std::min(std::min(smax, L2_SMAX), L2_SHM_BUDGET / (L2S_WARPS * 32) - 2) : 0;
+              // (the switch l2_fast = 0 sends every candidate to l2_kernel)
+              lp.sLimit = (ctx->flags.l2Fast && cmw >= 2 && ix->cmw == cmw && ix->rec8.p) ? std::min(std::min(smax, L2_SMAX), L2_SHM_BUDGET / (L2S_WARPS * 32) - 2) : 0;
               // bucket width near 0 ~ 2^32 / (s * w): minimizer hashes are minima of w hashes, density w/2^32 at 0
               lp.nBuckets = ((uint64_t)C >= 8ull * (uint64_t)F) ? L2E_BUCKETS : 1024;      // few candidates per fragment: building a big directory is not worth it
               { const int forced = ctx->flags.l2eBuckets;
@@ -1609,6 +1635,7 @@ void qsketch_map(Ctx *ctx, const Index *ix, const QSketch *const *sketches, int3
               lp.cB0 = cB0.p; lp.cE0 = cE0.p; lp.cLast = cLast.p; lp.cNEv = cNEv.p; lp.cChunks = cChunks.p; lp.cOff = cOff.p;
               lp.cPos = cPos.p; lp.cBest = cBest.p; lp.ctr_n2 = d_n2.p; lp.events = nullptr; lp.perm = nullptr;
               l2_bounds_kernel<<<nblk((uint64_t)C + 1), 256, 0, st>>>(lp); ctx->launches++;
+              if (countPaths) pp[P_L2_EXACT_AT_BOUNDS] += count_exact(ctx, cBest.p, C);
               if (lp.sLimit > 0) {
                 // candidates by descending event count: rank g -> warp g / 32, lane g % 32 of the sequential kernel
                 BANI_SCRATCH(uint32_t, skey, C);
@@ -1633,11 +1660,11 @@ void qsketch_map(Ctx *ctx, const Index *ix, const QSketch *const *sketches, int3
                 BANI_CUDA(cudaMemcpyAsync(&totalGrpSteps, grpOff.p + nGrp, 8, cudaMemcpyDeviceToHost, st));
                 BANI_CUDA(cudaStreamSynchronize(st));
                 totalSteps = totalGrpSteps * 32;                      // 32-byte slots
-                if ((double)totalSteps * 32.0 > 0.25 * (double)ctx->memTotal && nQc > 1) {
+                if ((double)totalSteps * 32.0 > evLimit && nQc > 1) {
                   // the event streams of this piece would take more than a quarter of the device (small windows make many
                   // events per hit): map its halves instead, so that they fit beside the index
                   out.ctr.hits -= N; out.ctr.candidates -= C;
-                  split_in_halves();
+                  split_in_halves(P_PIECE_SPLIT_EVENTS);
                   goto piece_done;
                 }
                 if (totalSteps > 0xfffffff0ull) fail(BANI_ERR_LIMIT, "query chunk schedules more than 2^36 window events");
@@ -1646,6 +1673,18 @@ void qsketch_map(Ctx *ctx, const Index *ix, const QSketch *const *sketches, int3
                 l2_stream_base_kernel<<<nblk(C), 256, 0, st>>>(perm.p, grpOff.p, C, cOff.p); ctx->launches++;
                 // CTA size of the events kernel by candidates per fragment (warp per candidate: no idle warps in small shards)
                 const int evNT = ((uint64_t)C >= 6ull * (uint64_t)F) ? 256 : ((uint64_t)C >= 3ull * (uint64_t)F) ? 128 : 64;
+                if (countPaths) {
+                  // candidates with window events, by the variant of l2_events_kernel that writes them
+                  std::vector<uint32_t> nEv(C); std::vector<uint16_t> mb(C);
+                  BANI_CUDA(cudaMemcpyAsync(nEv.data(), cNEv.p, 4 * (size_t)C, cudaMemcpyDeviceToHost, st));
+                  BANI_CUDA(cudaMemcpyAsync(mb.data(), cMB.p, 2 * (size_t)C, cudaMemcpyDeviceToHost, st));
+                  BANI_CUDA(cudaStreamSynchronize(st));
+                  uint64_t withEv = 0, staged = 0;
+                  for (uint32_t c = 0; c < C; c++) if (nEv[c]) { withEv++; staged += mb[c] != 0xFFFFu; }
+                  pp[evNT == 256 ? P_L2_EVENTS_NT256 : evNT == 128 ? P_L2_EVENTS_NT128 : P_L2_EVENTS_NT64] += withEv;
+                  pp[lp.nBuckets == L2E_BUCKETS ? P_L2_DIR4096 : P_L2_DIR1024] += withEv;
+                  pp[P_L2_STAGED] += staged; pp[P_L2_DIRECT] += withEv - staged;
+                }
                 const size_t shmE = 4 * ((size_t)(evNT / 32) * (L2E_RING / 2) + (size_t)lp.sLimit + 4 + L2E_BUCKETS + 4 + 2) + 8 * ((size_t)lp.sLimit + 4) + 16;
                 const size_t shmS = (size_t)L2S_WARPS * lp.warpBytes;
                 if (shmE > (size_t)L2_SHM_BUDGET || shmS > (size_t)L2_SHM_BUDGET) fail(BANI_ERR_INTERNAL, "L2 shared-memory budget exceeded");
@@ -1666,6 +1705,7 @@ void qsketch_map(Ctx *ctx, const Index *ix, const QSketch *const *sketches, int3
                   l2_seq_kernel<<<nblk(C, L2S_WARPS * 32), L2S_WARPS * 32, shmS, st>>>(lp); ctx->launches++; }
               }
               sgb.stop();
+              if (countPaths) pp[P_L2_EXACT_TOTAL] += count_exact(ctx, cBest.p, C);
               // exact slow path for whatever the fast path flagged (counter overflow, very large sketches)
               Stage sgs(ctx, "l2_exact");
               l2_kernel<<<blocks, 64, 0, st>>>(l2); ctx->launches++;
@@ -1718,7 +1758,7 @@ void qsketch_map(Ctx *ctx, const Index *ix, const QSketch *const *sketches, int3
                     const int nPass = std::min<int>((int)tableQ, nQc - qa);
                     ca.qLo = qa; ca.qHi = qa + nPass;
                     cgi_scatter_kernel<<<nblk(R), 256, 0, st>>>(ca);
-                    ctx->launches++;
+                    ctx->launches++; pp[P_CGI_PASSES]++;
                     cgi_sum_kernel<<<nblk((uint64_t)nPass * nG), 256, 0, st>>>(table.p, touched.p, ix->contigBinOff.p, d_gce.p,
                                                                              ix->totalBins, nG, nPass, oCount.p + (size_t)qa * nG, oIdent.p + (size_t)qa * nG);
                     ctx->launches++;
@@ -1738,6 +1778,10 @@ void qsketch_map(Ctx *ctx, const Index *ix, const QSketch *const *sketches, int3
       BANI_CUDA(cudaStreamSynchronize(st));
     }
     if (!split) { out.ctr.fragments += F; out.ctr.sum_s += (F > 0 && ix->M > 0) ? T : 0; }
+    if (!split && countPaths) {
+      pp[P_PIECE_MAPPED]++;
+      for (int i = 0; i < NPATH; i++) ctx->paths[i] += pp[i];
+    }
     if (wantCgi && !split) {
       append_cgi_rows(hCount.data(), hIdent.data(), nQc, nG, qs->queryId.data() + q0, qs->totalFragments.data() + q0, out.cgi);
     }

@@ -117,10 +117,26 @@ BANI_API void *bani_ctx_stream(bani_ctx *ctx);
 /* Run-time switches of a context.  name: "sketch_reuse" (1 = read the fragment sketches of index members from the
  * index, 0 = always hash the query fragments: what a run with --ql != --rl does), "max_hits_per_piece",
  * "frag_l1_max", "l2e_buckets", "l2_stage", "upload_group_words" (tuning / test switches; results never depend on them).
+ * A "frag_l1_max" below 8192 sends fragments with more hits to the device-wide sort instead of one CTA each.
  * Environment, read when a context is created: BANI_NO_SKETCH_REUSE, BANI_MAX_HITS_PER_PIECE, BANI_FRAG_L1_MAX,
  * BANI_L2E_BUCKETS, BANI_L2_STAGE set the defaults of those switches; BANI_TRACE=1 prints the host wall clock between
- * marks of the orchestration (index build, query sketches, every piece of the mapping) on stderr. */
+ * marks of the orchestration (index build, query sketches, every piece of the mapping) on stderr.
+ * Switches that bring branches which otherwise need very large inputs down to test size (results never depend on them):
+ * "frags_per_piece" (1 .. 2^18, default 2^18: fragments per query piece; exported sketches do not depend on it),
+ * "event_bytes_per_piece" (0 = a quarter of device memory: a piece whose L2 event streams take more is mapped in halves),
+ * "cgi_table_queries" (0 = as many as 3 GiB of bin table hold: queries per pass of the identity reduction),
+ * "l2_fast" (1; 0 sends every L2 candidate to the exact kernel).  "count_paths" (default 0) turns on the branch counters
+ * of bani_ctx_path_counts; with it off the mapping launches exactly the same kernels with the same work. */
 BANI_API int  bani_ctx_set_flag(bani_ctx *ctx, const char *name, int64_t value);
+
+/* Which branches of the mapping path ran since the last call (counted only while the switch "count_paths" is on):
+ * fills up to n_max (name, count) pairs -- names in buffers of 32 chars, always the same list in the same order --
+ * sets *n, and clears the counters.  Counters: l1.class0 .. l1.class12 and l1.device_wide (fragments per L1 size class),
+ * lookup.walk_saturated / lookup.walk_full_bucket (probes that walked the sorted keys), l2.events_nt64|128|256,
+ * l2.dir1024|4096, l2.staged, l2.direct (L2 candidates with window events, per event-kernel variant), l2.exact_at_bounds /
+ * l2.exact_total (candidates left to the exact kernel after the bounds pass / in all), piece.mapped, piece.split_hits,
+ * piece.split_events, cgi.passes.  All but piece.split_* describe the pieces that were mapped, not those split. */
+BANI_API int  bani_ctx_path_counts(bani_ctx *ctx, char (*names)[32], uint64_t *counts, int32_t n_max, int32_t *n);
 
 /* Per-stage device timing.  When enabled, every stage of HP1/HP2 is bracketed by CUDA events on
  * the context's stream; bani_ctx_profile_read() synchronises, sums the elapsed time, launch count and
