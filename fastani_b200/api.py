@@ -109,6 +109,18 @@ def load_library():
         "bani_map_cgi_sketch": (C.c_int, [vp, vp, P(vp), i32, P(vp), P(u64), P(MapCounters)]),
         "bani_free": (None, [vp]),
         "bani_synth_genome": (C.c_int, [vp, u64, u32, u32, u32, i64, vp]),
+        "bani_index_build_budget": (C.c_int, [vp, P(vp), i32, u64, P(vp), P(i32), P(u64)]),
+        "bani_ctx_mem_stats": (C.c_int, [vp, P(u64), P(u64), P(u64)]),
+        "bani_ctx_trim": (C.c_int, [vp]),
+        "bani_ctx_plan_run": (C.c_int, [vp, u64, u64, vp, vp, i32, vp, vp, i32, vp, P(i32), vp, P(i32), P(u64)]),
+        "bani_plan_run": (C.c_int, [u64, u64, i64, i64, u64, u64, i32, i32, i32, vp, vp, i32, vp, vp, i32, vp, P(i32), vp, P(i32), P(u64)]),
+        "bani_run_working_set": (C.c_int, [u64, i64, i64, u64, u64, i32, u64, i32, i32, i32, P(u64)]),
+        "bani_index_footprint": (C.c_int, [u64, u64, u64, u64, u64, P(u64), P(u64)]),
+        "bani_map_working_set": (C.c_int, [u64, i64, i64, P(u64)]),
+        "bani_index_budget": (C.c_int, [u64, u64, u64, i32, P(u64)]),
+        "bani_plan_chunks": (C.c_int, [vp, vp, i32, i32, i32, u64, vp, P(i32)]),
+        "bani_qsketch_bytes_estimate": (C.c_int, [u64, i32, i32, P(u64)]),
+        "bani_parse_byte_count": (C.c_int, [C.c_char_p, P(u64)]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)          # AttributeError if the ABI lost a symbol
@@ -126,7 +138,9 @@ EXPORTED_SYMBOLS = [
     "bani_index_destroy", "bani_index_stats", "bani_index_minimizers", "bani_index_save", "bani_index_load", "bani_index_contigs",
     "bani_qsketch_from_index", "bani_index_lookup", "bani_map_genome",
     "bani_map_cgi", "bani_free", "bani_synth_genome", "bani_qsketch_create", "bani_qsketch_destroy", "bani_qsketch_info",
-    "bani_qsketch_export", "bani_qsketch_import", "bani_qsketch_merge", "bani_map_cgi_sketch"]
+    "bani_qsketch_export", "bani_qsketch_import", "bani_qsketch_merge", "bani_map_cgi_sketch",
+    "bani_index_build_budget", "bani_ctx_mem_stats", "bani_ctx_trim", "bani_ctx_plan_run", "bani_plan_run", "bani_run_working_set", "bani_index_footprint",
+    "bani_map_working_set", "bani_index_budget", "bani_plan_chunks", "bani_qsketch_bytes_estimate", "bani_parse_byte_count"]
 
 
 def _check(rc):
@@ -203,7 +217,8 @@ class Context:
 
     def set_flag(self, name, value):
         """bani_ctx_set_flag: "sketch_reuse", "max_hits_per_piece", "frag_l1_max", "l2e_buckets", "l2_stage",
-        "upload_group_words", "frags_per_piece", "event_bytes_per_piece", "cgi_table_queries", "l2_fast", "count_paths"."""
+        "upload_group_words", "frags_per_piece", "event_bytes_per_piece", "cgi_table_queries", "l2_fast", "count_paths",
+        "index_bytes_budget", "query_sketch_budget"."""
         _check(self.lib.bani_ctx_set_flag(self.h, name.encode(), int(value)))
 
     def path_counts(self):
@@ -213,6 +228,22 @@ class Context:
         cnt = (C.c_uint64 * nmax)(); n = C.c_int32()
         _check(self.lib.bani_ctx_path_counts(self.h, names, cnt, nmax, C.byref(n)))
         return {names[i].value.decode(): int(cnt[i]) for i in range(n.value)}
+
+    def mem_stats(self):
+        """{"live", "cached", "peak_live"} device bytes of this context's device (bani_ctx_mem_stats; the peak is reset)."""
+        a = [C.c_uint64() for _ in range(3)]
+        _check(self.lib.bani_ctx_mem_stats(self.h, *[C.byref(x) for x in a]))
+        return dict(zip(("live", "cached", "peak_live"), [x.value for x in a]))
+
+    def trim(self):
+        """Drops the scratch slots and returns every cached block of the device to the driver (bani_ctx_trim)."""
+        _check(self.lib.bani_ctx_trim(self.h))
+
+    def plan_run(self, ref_lengths, ref_contigs, query_lengths, query_sketch_bytes=None, index_budget=0, query_budget=0):
+        """bani_ctx_plan_run with this context's free device memory: ([(first, end)] reference chunks, [(first, end)]
+        query blocks, index budget).  index_budget / query_budget (bytes) override the context's switches when not 0."""
+        return _plan_run(lambda *a: self.lib.bani_ctx_plan_run(self.h, int(index_budget), int(query_budget), *a),
+                         ref_lengths, ref_contigs, query_lengths, query_sketch_bytes)
 
     def profile(self, on=True):
         _check(self.lib.bani_ctx_profile_enable(self.h, 1 if on else 0))
@@ -404,6 +435,20 @@ class Sketch:
         self.metadata = [m for g in self.refs for m in g.metadata]                  # winSketch.hpp:66
         self.sequencesByFileInfo = list(np.cumsum([len(g.metadata) for g in self.refs]).astype(int))   # :75
 
+    @classmethod
+    def build_budget(cls, ctx, ref_genomes, max_bytes):
+        """bani_index_build_budget: the index of the longest prefix of ref_genomes whose build fits max_bytes (at least one
+        genome).  Returns (Sketch, n_taken, peak_bytes)."""
+        refs = list(ref_genomes)
+        arr = (C.c_void_p * max(len(refs), 1))(*[g.h for g in refs])
+        h = C.c_void_p(); n = C.c_int32(); peak = C.c_uint64()
+        _check(ctx.lib.bani_index_build_budget(ctx.h, arr, len(refs), int(max_bytes), C.byref(h), C.byref(n), C.byref(peak)))
+        sk = cls(ctx, None, _handle=h)
+        sk.refs = refs[:n.value]
+        sk.metadata = [m for g in sk.refs for m in g.metadata]
+        sk.sequencesByFileInfo = list(np.cumsum([len(g.metadata) for g in sk.refs]).astype(int))
+        return sk, n.value, peak.value
+
     def save(self, path):
         """On-disk sketch cache (bani_index_save): records + contig table + parameters; names are the caller's."""
         _check(self.ctx.lib.bani_index_save(self.ctx.h, self.h, os.fsencode(path)))
@@ -580,3 +625,135 @@ def compute_cgi_sketched(ctx, refSketch, query_sketches):
     else:
         out = np.empty(0, CGI_DTYPE)
     return out, ctr
+
+
+# ---------------------------------------------------------------------------------------- chunked runs
+def index_footprint(n_minimizers, n_unique_bound, n_contigs, bitmap_bits, staging_cap):
+    """(build peak, resident index) in device bytes of an index build (bani_index_footprint; no GPU needed)."""
+    pk, rs = C.c_uint64(), C.c_uint64()
+    _check(load_library().bani_index_footprint(int(n_minimizers), int(n_unique_bound), int(n_contigs), int(bitmap_bits),
+                                               int(staging_cap), C.byref(pk), C.byref(rs)))
+    return pk.value, rs.value
+
+
+def map_working_set(device_bytes, max_hits_per_piece=3 << 29, event_bytes_per_piece=0):
+    """Device bytes of the mapping working set from its caps (bani_map_working_set; no GPU needed)."""
+    b = C.c_uint64()
+    _check(load_library().bani_map_working_set(int(device_bytes), int(max_hits_per_piece), int(event_bytes_per_piece), C.byref(b)))
+    return b.value
+
+
+def index_budget(free_bytes, query_sketch_bytes, working_set, window_size):
+    """The index budget (bani_index_budget; no GPU needed)."""
+    b = C.c_uint64()
+    _check(load_library().bani_index_budget(int(free_bytes), int(query_sketch_bytes), int(working_set), int(window_size), C.byref(b)))
+    return b.value
+
+
+def plan_chunks(genome_lengths, genome_contigs, k, w, budget):
+    """Consecutive chunks [(first, end)] of a reference list whose indexes fit `budget` (bani_plan_chunks; no GPU needed).
+    Raises BaniError (BANI_ERR_LIMIT) naming a genome that alone does not fit."""
+    ln = np.ascontiguousarray(genome_lengths, dtype=np.uint64)
+    nc = np.ascontiguousarray(genome_contigs, dtype=np.int32)
+    assert len(ln) == len(nc)
+    ends = np.zeros(max(len(ln), 1), np.int32); n = C.c_int32()
+    _check(load_library().bani_plan_chunks(ln.ctypes.data, nc.ctypes.data, len(ln), int(k), int(w), int(budget),
+                                           ends.ctypes.data, C.byref(n)))
+    return _ranges(ends[:n.value].tolist())
+
+
+def parse_byte_count(text):
+    """How BANI_INDEX_BUDGET / BANI_QUERY_BUDGET are read ("123", "64M", "2G"); raises BaniError otherwise."""
+    b = C.c_uint64()
+    _check(load_library().bani_parse_byte_count(text.encode(), C.byref(b)))
+    return b.value
+
+
+def _ranges(ends):
+    out, a = [], 0
+    for e in ends:
+        out.append((a, e)); a = e
+    return out
+
+
+def _plan_run(call, ref_lengths, ref_contigs, query_lengths, query_sketch_bytes):
+    rl = np.ascontiguousarray(ref_lengths, dtype=np.uint64)
+    rc = np.ascontiguousarray(ref_contigs, dtype=np.int32)
+    ql = np.ascontiguousarray(query_lengths, dtype=np.uint64)
+    qb = None if query_sketch_bytes is None else np.ascontiguousarray(query_sketch_bytes, dtype=np.uint64)
+    assert len(rl) == len(rc) and (qb is None or len(qb) == len(ql))
+    ce = np.zeros(max(len(rl), 1), np.int32); be = np.zeros(max(len(ql), 1), np.int32)
+    nc, nb, ib = C.c_int32(), C.c_int32(), C.c_uint64()
+    _check(call(rl.ctypes.data, rc.ctypes.data, len(rl), ql.ctypes.data, qb.ctypes.data if qb is not None else None, len(ql),
+                ce.ctypes.data, C.byref(nc), be.ctypes.data, C.byref(nb), C.byref(ib)))
+    return _ranges(ce[:nc.value].tolist()), _ranges(be[:nb.value].tolist()), ib.value
+
+
+def plan_run(free_bytes, device_bytes, ref_lengths, ref_contigs, query_lengths, query_sketch_bytes=None, k=16, w=24, frag_len=3000,
+             index_budget=0, query_budget=0, max_hits_per_piece=3 << 29, event_bytes_per_piece=0):
+    """bani_plan_run (no GPU needed): ([(first, end)] reference chunks, [(first, end)] query blocks, index budget) of one GPU's
+    run with free_bytes of device memory free.  Budgets of 0 are derived; a derived budget that cannot hold a genome plans
+    the run on one index, a forced one raises BaniError naming the genome."""
+    return _plan_run(lambda *a: load_library().bani_plan_run(int(free_bytes), int(device_bytes), int(max_hits_per_piece),
+                                                             int(event_bytes_per_piece), int(index_budget), int(query_budget),
+                                                             int(k), int(w), int(frag_len), *a),
+                     ref_lengths, ref_contigs, query_lengths, query_sketch_bytes)
+
+
+def run_working_set(device_bytes, query_hashes, query_fragments, n_queries, ref_bases, n_refs, w=24, frag_len=3000,
+                    max_hits_per_piece=3 << 29, event_bytes_per_piece=0):
+    """The mapping working set a run of this size can reach (bani_run_working_set; no GPU needed)."""
+    b = C.c_uint64()
+    _check(load_library().bani_run_working_set(int(device_bytes), int(max_hits_per_piece), int(event_bytes_per_piece), int(query_hashes),
+                                               int(query_fragments), int(n_queries), int(ref_bases), int(n_refs), int(w), int(frag_len),
+                                               C.byref(b)))
+    return b.value
+
+
+def compute_cgi_chunked(ctx, ref_contig_lists, query_sketches, index_budget=None, query_budget=None):
+    """compute_cgi_sketched against a reference list that need not fit the device at once: Context.plan_run cuts the
+    references into chunks and the query sketches into blocks (each sketch counts as one query of its hashes' expected
+    length); every chunk is uploaded, indexed (bani_index_build_budget: genomes it does not take stay uploaded for the
+    next chunk) and mapped against every block.  refGenomeId is the position in ref_contig_lists.  Budgets (bytes)
+    default to the context's switches, else to what its free device memory allows.  A run of one chunk and one block is
+    compute_cgi_sketched on one index.
+    Returns (results[CGI_DTYPE] ordered by (query, ref), plan) with plan = {"chunks": [(first, end)] per index built,
+    "blocks": [(first, end)] ranges of query_sketches, "index_budget", "device_bytes": live + cached device bytes after
+    every chunk}."""
+    refs = list(ref_contig_lists)
+    qs = list(query_sketches)
+    infos = [q.info() for q in qs]
+    qlen = [x["n_hashes"] * (ctx.windowSize + 1) // 2 for x in infos]
+    lens = [sum(len(c[1] if isinstance(c, tuple) else c) for c in cl) for cl in refs]
+    planned, blocks, ib = ctx.plan_run(lens, [len(cl) for cl in refs], qlen, [x["export_bytes"] for x in infos],
+                                       index_budget or 0, query_budget or 0)
+    plan = {"chunks": [], "blocks": blocks, "index_budget": ib, "device_bytes": []}
+    if len(planned) <= 1 and len(blocks) <= 1:                    # fits: one index, one mapping call
+        sk = Sketch(ctx, ctx.genomes(refs))
+        res, _ = compute_cgi_sketched(ctx, sk, qs)
+        plan["chunks"] = [(0, len(refs))]
+        return res, plan
+    parts = []
+    for bi, (q0, q1) in enumerate(blocks):
+        nxt, pending, first = 0, [], 0
+        while nxt < len(planned) or pending:
+            if not pending:
+                a, e = planned[nxt]; nxt += 1
+                pending, first = ctx.genomes(refs[a:e]), a
+            sk, taken, _ = Sketch.build_budget(ctx, pending, ib)
+            for g in pending[:taken]:
+                g.close()
+            pending = pending[taken:]
+            res, _ = compute_cgi_sketched(ctx, sk, qs[q0:q1])
+            res["refGenomeId"] += first
+            parts.append(res)
+            sk.close()
+            ctx.trim()
+            if bi == 0:
+                plan["chunks"].append((first, first + taken))
+                m = ctx.mem_stats()
+                plan["device_bytes"].append(m["live"] + m["cached"])
+            first += taken
+    out = np.concatenate(parts) if parts else np.empty(0, CGI_DTYPE)
+    out = out[np.lexsort((out["refGenomeId"], out["qryGenomeId"]))]
+    return out, plan

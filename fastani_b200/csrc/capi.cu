@@ -104,6 +104,15 @@ int bani_ctx_create(int device, const bani_params *p, bani_ctx **out)
     if (const char *e = getenv("BANI_L2_STAGE")) f.l2Stage = atoi(e) != 0;
     if (const char *e = getenv("BANI_TRACE")) f.trace = atoi(e) != 0;
     if (const char *e = getenv("BANI_L2E_BUCKETS")) { const int v = atoi(e); if (v == 1024 || v == 4096) f.l2eBuckets = v; }
+    uint64_t b = 0;
+    if (const char *e = getenv("BANI_INDEX_BUDGET")) {
+      if (!parse_byte_count(e, &b)) fail(BANI_ERR_ARG, "BANI_INDEX_BUDGET=%s is not a byte count (digits, optionally followed by K, M or G)", e);
+      f.indexBytesBudget = b;
+    }
+    if (const char *e = getenv("BANI_QUERY_BUDGET")) {
+      if (!parse_byte_count(e, &b)) fail(BANI_ERR_ARG, "BANI_QUERY_BUDGET=%s is not a byte count (digits, optionally followed by K, M or G)", e);
+      f.querySketchBudget = b;
+    }
   }
   dev_cache_flush(device);                   // blocks cached under streams of destroyed contexts
   BANI_CUDA(cudaStreamCreateWithFlags(&c->c.stream, cudaStreamNonBlocking));
@@ -162,6 +171,8 @@ int bani_ctx_set_flag(bani_ctx *ctx, const char *name, int64_t value)
   else if (n == "cgi_table_queries") { if (value < 0) fail(BANI_ERR_ARG, "cgi_table_queries must not be negative"); f.cgiTableQueries = value; }
   else if (n == "l2_fast") f.l2Fast = value != 0;
   else if (n == "count_paths") f.countPaths = value != 0;
+  else if (n == "index_bytes_budget") { if (value < 0) fail(BANI_ERR_ARG, "index_bytes_budget must not be negative"); f.indexBytesBudget = (unsigned long long)value; }
+  else if (n == "query_sketch_budget") { if (value < 0) fail(BANI_ERR_ARG, "query_sketch_budget must not be negative"); f.querySketchBudget = (unsigned long long)value; }
   else fail(BANI_ERR_ARG, "unknown flag '%s'", name);
   return BANI_OK;
   BANI_CATCH
@@ -225,6 +236,161 @@ int bani_ctx_profile_read(bani_ctx *ctx, char (*names)[32], double *ms, double *
 }
 
 uint64_t bani_ctx_launch_count(const bani_ctx *ctx) { return ctx ? ctx->c.launches : 0; }
+
+int bani_ctx_mem_stats(bani_ctx *ctx, uint64_t *live, uint64_t *cached, uint64_t *peak_live)
+{
+  BANI_TRY
+  if (!ctx) fail(BANI_ERR_ARG, "null context");
+  size_t l = 0, c = 0, p = 0;
+  dev_mem_stats(ctx->c.device, &l, &c, &p);
+  dev_mem_peak_set(ctx->c.device, 0);
+  if (live) *live = l;
+  if (cached) *cached = c;
+  if (peak_live) *peak_live = p;
+  return BANI_OK;
+  BANI_CATCH
+}
+
+int bani_ctx_trim(bani_ctx *ctx)
+{
+  BANI_TRY
+  if (!ctx) fail(BANI_ERR_ARG, "null context");
+  BANI_CUDA(cudaSetDevice(ctx->c.device));
+  BANI_CUDA(cudaStreamSynchronize(ctx->c.stream));
+  ctx->c.slots.clear();
+  dev_cache_flush(ctx->c.device);
+  return BANI_OK;
+  BANI_CATCH
+}
+
+static int plan_run_checked(const RunSize &r, const uint64_t *ref_len, const int32_t *ref_contigs, int32_t n_refs, const uint64_t *query_len,
+                            const uint64_t *query_sketch_bytes, int32_t n_queries, int32_t *chunk_end, int32_t *n_chunks, int32_t *block_end,
+                            int32_t *n_blocks, uint64_t *index_budget)
+{
+  if (n_refs < 0 || n_queries < 0 || (n_refs && (!ref_len || !ref_contigs || !chunk_end)) || (n_queries && (!query_len || !block_end)) ||
+      !n_chunks || !n_blocks || r.k < 1 || r.w < 1 || r.fragLen < 1)
+    fail(BANI_ERR_ARG, "bad argument");
+  uint64_t ib = 0;
+  const int32_t nc = plan_run(r, ref_len, ref_contigs, n_refs, query_len, query_sketch_bytes, n_queries, chunk_end, block_end, n_blocks, &ib);
+  if (nc < 0)
+    fail(BANI_ERR_LIMIT, "reference genome %d (%llu bases) alone does not fit the index budget of %llu bytes", -nc - 1,
+         (unsigned long long)ref_len[-nc - 1], (unsigned long long)ib);
+  *n_chunks = nc;
+  if (index_budget) *index_budget = ib;
+  return BANI_OK;
+}
+
+int bani_plan_run(uint64_t free_bytes, uint64_t device_bytes, int64_t max_hits_per_piece, int64_t event_bytes_per_piece,
+                  uint64_t index_budget, uint64_t query_budget, int32_t k, int32_t w, int32_t frag_len,
+                  const uint64_t *ref_len, const int32_t *ref_contigs, int32_t n_refs, const uint64_t *query_len,
+                  const uint64_t *query_sketch_bytes, int32_t n_queries, int32_t *chunk_end, int32_t *n_chunks,
+                  int32_t *block_end, int32_t *n_blocks, uint64_t *index_budget_used)
+{
+  BANI_TRY
+  RunSize r;
+  r.freeBytes = free_bytes; r.deviceBytes = device_bytes; r.maxHitsPerPiece = max_hits_per_piece; r.eventBytesPerPiece = event_bytes_per_piece;
+  r.indexBudget = index_budget; r.queryBudget = query_budget; r.k = k; r.w = w; r.fragLen = frag_len;
+  return plan_run_checked(r, ref_len, ref_contigs, n_refs, query_len, query_sketch_bytes, n_queries, chunk_end, n_chunks, block_end, n_blocks,
+                          index_budget_used);
+  BANI_CATCH
+}
+
+int bani_ctx_plan_run(bani_ctx *ctx, uint64_t index_budget, uint64_t query_budget, const uint64_t *ref_len, const int32_t *ref_contigs, int32_t n_refs, const uint64_t *query_len,
+                      const uint64_t *query_sketch_bytes, int32_t n_queries, int32_t *chunk_end, int32_t *n_chunks,
+                      int32_t *block_end, int32_t *n_blocks, uint64_t *index_budget_used)
+{
+  BANI_TRY
+  if (!ctx) fail(BANI_ERR_ARG, "null context");
+  BANI_CUDA(cudaSetDevice(ctx->c.device));
+  size_t freeB = 0, totalB = 0, cached = 0;
+  BANI_CUDA(cudaMemGetInfo(&freeB, &totalB));
+  dev_mem_stats(ctx->c.device, nullptr, &cached, nullptr);
+  const CtxFlags &f = ctx->c.flags;
+  RunSize r;
+  r.freeBytes = (uint64_t)freeB + (uint64_t)cached;                  // cached blocks go back to the driver on demand
+  r.deviceBytes = ctx->c.memTotal; r.maxHitsPerPiece = f.maxHitsPerPiece; r.eventBytesPerPiece = f.eventBytesPerPiece;
+  r.indexBudget = index_budget ? index_budget : f.indexBytesBudget; r.queryBudget = query_budget ? query_budget : f.querySketchBudget;
+  r.k = ctx->c.prm.kmer_size; r.w = ctx->c.prm.window_size; r.fragLen = ctx->c.prm.frag_len;
+  return plan_run_checked(r, ref_len, ref_contigs, n_refs, query_len, query_sketch_bytes, n_queries, chunk_end, n_chunks, block_end, n_blocks,
+                          index_budget_used);
+  BANI_CATCH
+}
+
+int bani_index_footprint(uint64_t n_minimizers, uint64_t n_unique_bound, uint64_t n_contigs, uint64_t bitmap_bits, uint64_t staging_cap,
+                         uint64_t *build_peak, uint64_t *resident)
+{
+  BANI_TRY
+  if (n_unique_bound > n_minimizers) fail(BANI_ERR_ARG, "more unique hashes than minimizers");
+  const IndexFootprint f = index_footprint(n_minimizers, n_unique_bound, n_contigs, bitmap_bits, staging_cap);
+  if (build_peak) *build_peak = f.peak;
+  if (resident) *resident = f.resident;
+  return BANI_OK;
+  BANI_CATCH
+}
+
+int bani_map_working_set(uint64_t device_bytes, int64_t max_hits_per_piece, int64_t event_bytes_per_piece, uint64_t *bytes)
+{
+  BANI_TRY
+  if (!bytes) fail(BANI_ERR_ARG, "null argument");
+  *bytes = map_working_set(device_bytes, max_hits_per_piece, event_bytes_per_piece);
+  return BANI_OK;
+  BANI_CATCH
+}
+
+int bani_run_working_set(uint64_t device_bytes, int64_t max_hits_per_piece, int64_t event_bytes_per_piece, uint64_t query_hashes,
+                         uint64_t query_fragments, int32_t n_queries, uint64_t ref_bases, int32_t n_refs, int32_t window_size,
+                         int32_t frag_len, uint64_t *bytes)
+{
+  BANI_TRY
+  if (!bytes || n_queries < 0 || n_refs < 0 || window_size < 1 || frag_len < 1) fail(BANI_ERR_ARG, "bad argument");
+  *bytes = map_working_set_run(device_bytes, max_hits_per_piece, event_bytes_per_piece, query_hashes, query_fragments, (uint64_t)n_queries,
+                               ref_bases, (uint64_t)n_refs, window_size, frag_len);
+  return BANI_OK;
+  BANI_CATCH
+}
+
+int bani_index_budget(uint64_t free_bytes, uint64_t query_sketch_bytes, uint64_t working_set, int32_t window_size, uint64_t *budget)
+{
+  BANI_TRY
+  if (!budget || window_size < 1) fail(BANI_ERR_ARG, "bad argument");
+  *budget = index_budget(free_bytes, query_sketch_bytes, working_set, window_size);
+  return BANI_OK;
+  BANI_CATCH
+}
+
+int bani_plan_chunks(const uint64_t *genome_len, const int32_t *genome_contigs, int32_t n, int32_t k, int32_t w, uint64_t budget,
+                     int32_t *chunk_end, int32_t *n_chunks)
+{
+  BANI_TRY
+  if (n < 0 || (n && (!genome_len || !genome_contigs || !chunk_end)) || !n_chunks || k < 1 || w < 1) fail(BANI_ERR_ARG, "bad argument");
+  const int32_t r = plan_chunks(genome_len, genome_contigs, n, k, w, budget, chunk_end);
+  if (r < 0) {
+    const int32_t g = -r - 1;
+    fail(BANI_ERR_LIMIT, "reference genome %d (%llu bases) alone does not fit the index budget of %llu bytes", g,
+         (unsigned long long)genome_len[g], (unsigned long long)budget);
+  }
+  *n_chunks = r;
+  return BANI_OK;
+  BANI_CATCH
+}
+
+int bani_qsketch_bytes_estimate(uint64_t len, int32_t w, int32_t frag_len, uint64_t *bytes)
+{
+  BANI_TRY
+  if (!bytes || w < 1) fail(BANI_ERR_ARG, "bad argument");
+  *bytes = qsketch_bytes_estimate(len, w, frag_len);
+  return BANI_OK;
+  BANI_CATCH
+}
+
+int bani_parse_byte_count(const char *s, uint64_t *out)
+{
+  BANI_TRY
+  if (!out) fail(BANI_ERR_ARG, "null argument");
+  if (!parse_byte_count(s, out)) fail(BANI_ERR_ARG, "'%s' is not a byte count (digits, optionally followed by K, M or G)", s ? s : "");
+  return BANI_OK;
+  BANI_CATCH
+}
 
 void *bani_ctx_stream(bani_ctx *ctx) { return ctx ? (void *)ctx->c.stream : nullptr; }
 
@@ -338,6 +504,23 @@ int bani_index_build(bani_ctx *ctx, bani_genome *const *refs, int32_t n_refs, ba
   for (int i = 0; i < n_refs; i++) { if (!refs[i]) fail(BANI_ERR_ARG, "null genome handle"); gs[i] = &refs[i]->g; }
   Index *ix = index_build(&ctx->c, gs.data(), n_refs);
   bani_index *h = new bani_index(); h->ix = ix; *out = h;
+  return BANI_OK;
+  BANI_CATCH
+}
+
+int bani_index_build_budget(bani_ctx *ctx, bani_genome *const *refs, int32_t n_refs, uint64_t max_bytes, bani_index **out,
+                            int32_t *n_taken, uint64_t *peak_bytes)
+{
+  BANI_TRY
+  if (!ctx || !out || !n_taken || n_refs < 1 || !refs) fail(BANI_ERR_ARG, "null argument");
+  BANI_CUDA(cudaSetDevice(ctx->c.device));
+  std::vector<Genome *> gs(n_refs);
+  for (int i = 0; i < n_refs; i++) { if (!refs[i]) fail(BANI_ERR_ARG, "null genome handle"); gs[i] = &refs[i]->g; }
+  int32_t taken = 0; uint64_t peak = 0;
+  Index *ix = index_build_budget(&ctx->c, gs.data(), n_refs, max_bytes, &taken, &peak);
+  bani_index *h = new bani_index(); h->ix = ix; *out = h;
+  *n_taken = taken;
+  if (peak_bytes) *peak_bytes = peak;
   return BANI_OK;
   BANI_CATCH
 }

@@ -38,6 +38,9 @@ void set_last_error(const std::string &m);
 void *dev_alloc(size_t bytes, cudaStream_t st, size_t *granted, int *dev);
 void  dev_free(void *p, size_t granted, cudaStream_t st, int dev);      // dev = the device the block was allocated on
 void  dev_cache_flush(int dev);
+size_t dev_round_size(size_t bytes);                                    // what a request of `bytes` is rounded to
+void  dev_mem_stats(int dev, size_t *live, size_t *cached, size_t *peakLive);
+void  dev_mem_peak_set(int dev, size_t v);                              // peakLive = max(v, live)
 
 template <typename T>
 struct DevBuf {
@@ -215,6 +218,9 @@ struct CtxFlags {
   long long cgiTableQueries = 0;              // queries per pass of the identity reduction; 0 = as many as 3 GiB of bin table hold
   int l2Fast = 1;                             // 0: every L2 candidate goes to the exact kernel (l2_kernel)
   int countPaths = 0;                         // 1: count which branch of the mapping path ran (bani_ctx_path_counts)
+  // Budgets of a run that builds its references in chunks (bani_ctx_plan_run); results never depend on them.
+  unsigned long long indexBytesBudget = 0;    // build peak of one chunk's index; 0 = derived from device memory
+  unsigned long long querySketchBudget = 0;   // query sketches resident at once; 0 = derived from device memory
 };
 
 // Branches of the mapping path, counted when CtxFlags::countPaths is set (names: capi.cu, bani_ctx_path_counts).  What a
@@ -320,6 +326,42 @@ uint64_t sketch_sequences(Ctx *ctx, const SeqDesc *d_desc, int32_t nSeq, const i
 
 // index.cu
 Index *index_build(Ctx *ctx, Genome *const *refs, int32_t nRefs);
+// The longest prefix of refs whose build peak (index_footprint) fits maxBytes, at least one genome (BANI_ERR_LIMIT if that
+// one does not fit); the index equals index_build's of exactly that prefix.  *peakBytes: most bytes held above the entry.
+Index *index_build_budget(Ctx *ctx, Genome *const *refs, int32_t nRefs, uint64_t maxBytes, int32_t *nTaken, uint64_t *peakBytes);
+
+// budget.cpp (host arithmetic only): index footprint, mapping working set, index budget, chunk plan
+inline int index_dir_bits(uint64_t U) { int b = 8; while (b < 23 && (1ull << b) < U) b++; return b; }    // <= 32 MB directory
+inline int index_tab_bits(uint64_t U) { int b = 8; while (b < 28 && (1ull << b) < U) b++; return b; }    // >= U buckets, <= 2^28
+inline int index_filt_bits(uint64_t U)                                                                  // 0 = no filter; <= 32 MB
+{
+  if (U > (1ull << 26)) return 0;
+  int fb = 8; while ((1ull << fb) < U) fb++;
+  return fb + 3 < 28 ? fb + 3 : 28;
+}
+// th/tw/ts capacity of index_build: 1.5x the expected 2 / (w + 1) minimizers per position
+inline uint64_t index_staging_cap(uint64_t totalPos, int w)
+{
+  const uint64_t c = (uint64_t)(3.0 * totalPos / (w + 1)) + 65536;
+  return c < totalPos ? c : totalPos;
+}
+struct IndexFootprint { uint64_t peak = 0, resident = 0; };
+IndexFootprint index_footprint(uint64_t M, uint64_t Ubound, uint64_t nContigs, uint64_t bitmapBits, uint64_t stagingCap);
+uint64_t map_working_set(uint64_t deviceBytes, long long maxHitsPerPiece, long long eventBytesPerPiece);
+uint64_t map_working_set_run(uint64_t deviceBytes, long long maxHitsPerPiece, long long eventBytesPerPiece, uint64_t queryHashes,
+                             uint64_t queryFragments, uint64_t nQueries, uint64_t refBases, uint64_t nRefs, int w, int fragLen);
+uint64_t index_budget(uint64_t freeBytes, uint64_t qsketchBytes, uint64_t workingSet, int w);
+int32_t  plan_chunks(const uint64_t *len, const int32_t *nContigs, int32_t n, int k, int w, uint64_t budget, int32_t *ends);
+uint64_t qsketch_bytes_estimate(uint64_t len, int w, int fragLen);
+// what a run plan depends on besides the genome sizes: free device bytes (free + cached), the device's size, the piece caps,
+// the forced budgets (0 = derived) and the parameters
+struct RunSize {
+  uint64_t freeBytes = 0, deviceBytes = 0; long long maxHitsPerPiece = 0, eventBytesPerPiece = 0;
+  uint64_t indexBudget = 0, queryBudget = 0; int k = 16, w = 1, fragLen = 3000;
+};
+int32_t plan_run(const RunSize &r, const uint64_t *refLen, const int32_t *refContigs, int32_t nRefs, const uint64_t *queryLen,
+                 const uint64_t *qsBytes, int32_t nQ, int32_t *chunkEnd, int32_t *blockEnd, int32_t *nBlocks, uint64_t *indexBudget);
+bool     parse_byte_count(const char *s, uint64_t *out);
 void   index_save(Ctx *ctx, const Index *ix, const char *path);
 Index *index_load(Ctx *ctx, const char *path);
 

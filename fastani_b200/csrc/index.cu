@@ -251,18 +251,17 @@ static void index_finish(Ctx *ctx, Index *ix)
   BANI_CUDA(cudaMemsetAsync(ix->link.p, 0xFF, 4 * (size_t)M, st));
   links_kernel<<<nblk(M), 256, 0, st>>>(sortedHash.p, ix->posIdx.p, M, ix->link.p);
   ctx->launches++;
-  int bits = 8; while (bits < 23 && (1ull << bits) < U) bits++;       // <= 32 MB: the directory stays L2-resident (50 MB) during a lookup launch
+  const int bits = index_dir_bits(U);       // <= 32 MB: the directory stays L2-resident (50 MB) during a lookup launch
   ix->dirBits = bits;
   ix->dir.alloc((1u << bits) + 1, st);
   dir_fill_kernel<<<nblk((1ull << bits) + 1), 256, 0, st>>>(ix->ukeys.p, (uint32_t)U, bits, ix->dir.p);
   ctx->launches++;
   {   // probe table: 2^tabBits >= U buckets (load <= 1 key per 4-slot bucket: ~2 % of the buckets are full), at most 2^28 (8.6 GB)
-    int tb = 8; while (tb < 28 && (1ull << tb) < U) tb++;
+    const int tb = index_tab_bits(U);
     ix->tabBits = tb;
     ix->tab.alloc((size_t)4 << tb, st);
     BANI_CUDA(cudaMemsetAsync(ix->tab.p, 0, ix->tab.bytes(), st));
-    int fb = 0;
-    if (U <= (1ull << 26)) { fb = 8; while ((1ull << fb) < U) fb++; fb = std::min(fb + 3, 28); }      // <= 32 MB of bits
+    const int fb = index_filt_bits(U);      // <= 32 MB of bits
     ix->filtBits = fb;
     if (fb) { ix->filt.alloc((size_t)1 << (fb - 5), st); BANI_CUDA(cudaMemsetAsync(ix->filt.p, 0, ix->filt.bytes(), st)); }
     table_fill_kernel<<<nblk(U), 256, 0, st>>>(ix->ukeys.p, ix->uoff.p, (uint32_t)U, (1u << tb) - 1u, ix->tab.p,
@@ -282,10 +281,101 @@ static void index_finish(Ctx *ctx, Index *ix)
   BANI_CUDA(cudaStreamSynchronize(st));
 }
 
-Index *index_build(Ctx *ctx, Genome *const *refs, int32_t nRefs)
+// Host sizes of genome g's part of an index: contigs, hashed positions (contigs of at least k bases) and validity bits.
+struct GenomeSpan { uint64_t nC = 0, pos = 0, bits = 0; };
+static GenomeSpan genome_span(const Genome *G, int k)
+{
+  GenomeSpan s;
+  s.nC = (uint64_t)G->nContigs;
+  for (int c = 0; c < G->nContigs; c++) {
+    if (G->len[c] >= k) s.pos += (uint64_t)(G->len[c] - k + 1);
+    s.bits += ((uint64_t)G->len[c] + 31) & ~31ull;
+  }
+  return s;
+}
+
+// Budgeted build, after the sketch launch over genomes [0, n): keeps the longest prefix whose records were all stored (<=
+// `stored`) and whose exact build (index_footprint with U <= M, the staging capacity that was used and the tables of all
+// launched genomes, which are alive until the cut) fits maxBytes, and
+// shrinks the contig tables, the genome table and the validity bitmap to it.  Returns the prefix's record count.
+static uint64_t index_cut(Ctx *ctx, Index *ix, Genome *const *refs, std::vector<int32_t> &contigGenome, const std::vector<GenomeSpan> &span,
+                          uint64_t stored, uint64_t cap, uint64_t maxBytes, int32_t *nTaken)
+{
+  cudaStream_t st = ctx->stream;
+  const int32_t n = (int32_t)ix->seqsByFile.size();
+  std::vector<uint32_t> recOff((size_t)ix->nContigs + 1);
+  BANI_CUDA(cudaMemcpyAsync(recOff.data(), ix->contigRecOff.p, 4 * recOff.size(), cudaMemcpyDeviceToHost, st));
+  BANI_CUDA(cudaStreamSynchronize(st));
+  // the contig tables and the bitmap of every launched genome stay alive until the cut: they are charged in full
+  uint64_t launchedBits = 0;
+  for (int32_t g = 0; g < n; g++) launchedBits += span[g].bits;
+  const uint64_t launchedC = (uint64_t)ix->nContigs;
+  int32_t t = 0;
+  uint64_t nC = 0, M = 0;
+  for (; t < n; t++) {
+    const uint64_t c2 = (uint64_t)ix->seqsByFile[t], m2 = recOff[c2];
+    if (m2 > stored || index_footprint(m2, m2, launchedC, launchedBits, cap).peak > maxBytes) break;
+    nC = c2; M = m2;
+  }
+  if (t == 0)
+    fail(BANI_ERR_LIMIT, "reference genome 0 of this chunk (%llu minimizers) does not fit the index budget of %llu bytes: its "
+         "index needs %llu", (unsigned long long)recOff[ix->seqsByFile[0]], (unsigned long long)maxBytes,
+         (unsigned long long)index_footprint(recOff[ix->seqsByFile[0]], recOff[ix->seqsByFile[0]], launchedC, launchedBits, cap).peak);
+  *nTaken = t;
+  if (t == n) return M;
+  // the prefix's tables, as index_build would have made them from exactly these genomes
+  ix->members.clear();
+  for (int32_t g = 0, c = 0; g < t; c += refs[g]->nContigs, g++) ix->members.emplace(refs[g]->uid, c);
+  ix->nGenomes = t;
+  ix->seqsByFile.resize(t);
+  ix->contigLen.resize(nC);
+  contigGenome.resize(nC);
+  DevBuf<uint32_t> oldRecOff = std::move(ix->contigRecOff);
+  DevBuf<uint32_t> oldBits = std::move(ix->validBits);
+  const unsigned long long totalBits = index_contig_tables(ctx, ix, contigGenome);     // totalBits == bits: whole words
+  BANI_CUDA(cudaMemcpyAsync(ix->contigRecOff.p, oldRecOff.p, 4 * (nC + 1), cudaMemcpyDeviceToDevice, st));
+  ix->validBits.alloc((size_t)(totalBits / 32) + 1, st);
+  BANI_CUDA(cudaMemsetAsync(ix->validBits.p, 0, ix->validBits.bytes(), st));
+  if (totalBits) BANI_CUDA(cudaMemcpyAsync(ix->validBits.p, oldBits.p, totalBits / 8, cudaMemcpyDeviceToDevice, st));
+  BANI_CUDA(cudaStreamSynchronize(st));
+  return M;
+}
+
+// maxBytes = 0: the whole list.  maxBytes > 0 (index_build_budget): the longest prefix whose build fits (*nTaken).
+//   Before the sketch launch only the expected record count is known: the launch takes the longest prefix whose expected
+//   build fits (at least one genome, whose staging and tables alone must fit).  After it, contigRecOff holds the exact
+//   record count of every genome; records are in (seqId, wpos) order, so a prefix of genomes is a prefix of the records,
+//   of the validity bitmap and of the contig tables, and the index is cut there before anything that grows with M or U
+//   is allocated.
+static Index *index_build_impl(Ctx *ctx, Genome *const *refs, int32_t nRefs, uint64_t maxBytes, int32_t *nTaken)
 {
   cudaStream_t st = ctx->stream;
   const int k = ctx->prm.kmer_size, w = ctx->prm.window_size, fragLen = ctx->prm.frag_len;
+  const bool budget = maxBytes > 0;
+  std::vector<GenomeSpan> span;
+  if (budget) {
+    for (int g = 0; g < nRefs; g++) {
+      if (!refs[g]) fail(BANI_ERR_ARG, "null genome handle");
+      span.push_back(genome_span(refs[g], k));
+    }
+    GenomeSpan p;
+    int32_t n = 0;
+    for (; n < nRefs; n++) {
+      GenomeSpan q = p; q.nC += span[n].nC; q.pos += span[n].pos; q.bits += span[n].bits;
+      const uint64_t cap = index_staging_cap(q.pos, w), Mexp = (uint64_t)(2.0 * (double)q.pos / (w + 1));
+      // genome 0: its staging and tables must fit (its records are counted after the launch); later genomes: the whole
+      // expected build
+      const uint64_t need = n == 0 ? index_footprint(0, 0, q.nC, q.bits, cap).peak : index_footprint(Mexp, Mexp, q.nC, q.bits, cap).peak;
+      if (need > maxBytes || (n > 0 && cap > 0xfffffff0ull)) break;
+      p = q;
+    }
+    if (n == 0)
+      fail(BANI_ERR_LIMIT, "reference genome 0 of this chunk (%llu bases) does not fit the index budget of %llu bytes: its sketch "
+           "staging alone needs %llu", (unsigned long long)span[0].pos, (unsigned long long)maxBytes,
+           (unsigned long long)index_footprint(0, 0, span[0].nC, span[0].bits, index_staging_cap(span[0].pos, w)).peak);
+    nRefs = n;
+  }
+  *nTaken = nRefs;
   auto ix = std::make_unique<Index>();
   ix->device = ctx->device;
   ix->nGenomes = nRefs;
@@ -328,7 +418,7 @@ Index *index_build(Ctx *ctx, Genome *const *refs, int32_t nRefs)
 
   // ---- build: minimizers in (seqId, wpos) order.  Expected density 2/(w+1); capacity 1.5x that,
   //      exact retry if a repetitive reference exceeds it (worst case one record per position).
-  uint64_t cap = std::min<uint64_t>(totalPos, (uint64_t)(3.0 * totalPos / (w + 1)) + 65536);
+  uint64_t cap = index_staging_cap(totalPos, w);
   uint64_t M = 0;
   {
     DevBuf<uint32_t> th; DevBuf<int32_t> tw, ts;
@@ -360,8 +450,23 @@ Index *index_build(Ctx *ctx, Genome *const *refs, int32_t nRefs)
       sg.bytes((double)ix->totalLen / 4.0 + 12.0 * (double)M);       // packed bases in, 12-byte records out
       ctx->mark("index_build: sketched");
       if (M <= cap) break;
+      if (budget) {
+        // only the genomes whose records were all stored can be kept: retry with an exact staging for genome 0 if even it
+        // overflowed the expected capacity
+        uint32_t r1 = 0;
+        BANI_CUDA(cudaMemcpyAsync(&r1, ix->contigRecOff.p + ix->seqsByFile[0], 4, cudaMemcpyDeviceToHost, st));
+        BANI_CUDA(cudaStreamSynchronize(st));
+        if (r1 <= cap) break;
+        if (index_footprint(r1, r1, (uint64_t)nC, totalBits, r1).peak > maxBytes)
+          fail(BANI_ERR_LIMIT, "reference genome 0 of this chunk (%llu minimizers) does not fit the index budget of %llu bytes",
+               (unsigned long long)r1, (unsigned long long)maxBytes);
+        cap = r1;
+        continue;
+      }
       cap = M;
     }
+    d_desc.release();                                             // the descriptors are only read by the sketch launch
+    if (budget) M = index_cut(ctx, ix.get(), refs, contigGenome, span, std::min(M, cap), cap, maxBytes, nTaken);
     if (M > 0xfffffff0ull) fail(BANI_ERR_LIMIT, "more than 2^32 minimizers in one index shard");
     ix->M = M;
     if (M == 0) { index_make_empty(ctx, ix.get()); return ix.release(); }
@@ -373,6 +478,28 @@ Index *index_build(Ctx *ctx, Genome *const *refs, int32_t nRefs)
   index_finish(ctx, ix.get());
   ctx->mark("index_build: finished");
   return ix.release();
+}
+
+Index *index_build(Ctx *ctx, Genome *const *refs, int32_t nRefs)
+{
+  int32_t n = 0;
+  return index_build_impl(ctx, refs, nRefs, 0, &n);
+}
+
+Index *index_build_budget(Ctx *ctx, Genome *const *refs, int32_t nRefs, uint64_t maxBytes, int32_t *nTaken, uint64_t *peakBytes)
+{
+  if (nRefs < 1) fail(BANI_ERR_ARG, "a budgeted index build needs at least one genome");
+  if (maxBytes == 0) fail(BANI_ERR_ARG, "the index budget must be positive");
+  size_t live0 = 0, peak0 = 0, peak = 0;
+  dev_mem_stats(ctx->device, &live0, nullptr, &peak0);
+  dev_mem_peak_set(ctx->device, 0);                        // high-water mark from here on
+  Index *ix = nullptr;
+  try { ix = index_build_impl(ctx, refs, nRefs, maxBytes, nTaken); }
+  catch (...) { dev_mem_stats(ctx->device, nullptr, nullptr, &peak); dev_mem_peak_set(ctx->device, std::max(peak0, peak)); throw; }
+  dev_mem_stats(ctx->device, nullptr, nullptr, &peak);
+  dev_mem_peak_set(ctx->device, std::max(peak0, peak));
+  *peakBytes = peak > live0 ? peak - live0 : 0;
+  return ix;
 }
 
 // ---------------------------------------------------------------------------------------- on-disk sketch cache (SURVEY 8 f-4)

@@ -203,17 +203,21 @@ class Sketch {
   bool sanityCheck(float maxRatioDiff)
   {
     if (!param_.sanityCheck) return true;
+    return indexSanityCheck(ix_, maxRatioDiff, ratioDifference_);
+  }
+  // the same for any index (a chunk of a reference shard): ratioDifference is set
+  static bool indexSanityCheck(const bani_index *ix, float maxRatioDiff, float &ratioDifference)
+  {
     uint64_t nMin = 0, nUniq = 0, totalLen = 0, nc = 0, ng = 0;
-    check(bani_index_stats(ix_, &nMin, &nUniq, &totalLen, &nc, &ng), "bani_index_stats");
-    hashRatio_ = float(totalLen) / float(nMin);
-    uniqHashRatio_ = float(totalLen) / float(nUniq);
-    ratioDifference_ = std::abs(hashRatio_ - uniqHashRatio_);
-    return !(ratioDifference_ > maxRatioDiff);
+    check(bani_index_stats(ix, &nMin, &nUniq, &totalLen, &nc, &ng), "bani_index_stats");
+    const float hashRatio = float(totalLen) / float(nMin), uniqHashRatio = float(totalLen) / float(nUniq);
+    ratioDifference = std::abs(hashRatio - uniqHashRatio);
+    return !(ratioDifference > maxRatioDiff);
   }
   float getRatioDifference() const { return ratioDifference_; }
  private:
   bani_ctx *ctx_; Parameters param_; bani_index *ix_ = nullptr;
-  float hashRatio_ = 0, uniqHashRatio_ = 0, ratioDifference_ = 1.0f;   // the reference leaves it uninitialised; it prints `true`
+  float ratioDifference_ = 1.0f;          // the reference leaves it uninitialised; it prints `true`
 };
 
 // ---------------------------------------------------------------------------------------- Map (HP2)

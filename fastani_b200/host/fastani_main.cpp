@@ -264,11 +264,113 @@ int main(int argc, char **argv)
     std::vector<std::vector<std::string>> savedContigNames(G);
     std::mutex mu; std::string err;
 
+    std::vector<std::vector<std::string>> chunkSanity(G);             // -s verdicts of chunked shards ("SPLIT g chunk c ...")
+
+    // A shard whose index does not fit the device at once.  Per query block: the block's queries are uploaded, hashed into
+    // sketches (no index to derive them from: every query is hashed) and their device genomes freed; then the shard's
+    // references are walked in chunks -- upload the planned genomes, build the longest prefix that fits the index budget
+    // (genomes it did not take stay uploaded for the next chunk), free the chunk's genomes, map, and hand the index and the
+    // cached blocks back before the next chunk.  Results carry shard-local reference ordinals, as those of one index would.
+    auto chunkedShard = [&](bani_ctx *ctx, int g, const std::vector<int> &shard, const std::vector<std::pair<int, int>> &chunks,
+                            const std::vector<std::pair<int, int>> &blocks, uint64_t indexBudget, std::vector<cgi::CGI_Results> &local) {
+      const int threads = std::max(1, parameters.threads / G);
+      int chunkNo = 0;
+      for (size_t b = 0; b < blocks.size(); b++) {
+        std::vector<const bani_host::HostGenome *> qh;
+        for (int q = blocks[b].first; q < blocks[b].second; q++) qh.push_back(&genomes[pathId.at(parameters.querySequences[q])]);
+        bani_qsketch *qsk = nullptr;
+        {
+          std::vector<std::unique_ptr<DeviceGenome>> dq;
+          upload_genomes(ctx, qh, dq, (size_t)1 << 28, threads);
+          std::vector<bani_genome *> hs; std::vector<int32_t> ids;
+          for (size_t i = 0; i < dq.size(); i++) { hs.push_back(dq[i]->h); ids.push_back(blocks[b].first + (int32_t)i); }
+          check(bani_qsketch_create(ctx, hs.data(), (int32_t)hs.size(), ids.data(), nullptr, &qsk), "bani_qsketch_create");
+        }
+        std::unique_ptr<bani_qsketch, void (*)(bani_qsketch *)> qskOwner(qsk, bani_qsketch_destroy);
+        std::vector<std::unique_ptr<DeviceGenome>> pending;
+        int first = 0;
+        size_t next = 0;
+        while (next < chunks.size() || !pending.empty()) {
+          if (pending.empty()) {
+            std::vector<const bani_host::HostGenome *> rh;
+            for (int i = chunks[next].first; i < chunks[next].second; i++) rh.push_back(&genomes[pathId.at(parameters.refSequences[shard[i]])]);
+            upload_genomes(ctx, rh, pending, (size_t)1 << 28, threads);
+            first = chunks[next].first;
+            next++;
+          }
+          std::vector<bani_genome *> hs; for (auto &d : pending) hs.push_back(d->h);
+          bani_index *ix = nullptr; int32_t taken = 0; uint64_t peak = 0;
+          check(bani_index_build_budget(ctx, hs.data(), (int32_t)hs.size(), indexBudget, &ix, &taken, &peak), "bani_index_build_budget");
+          std::unique_ptr<bani_index, void (*)(bani_index *)> ixOwner(ix, bani_index_destroy);
+          pending.erase(pending.begin(), pending.begin() + taken);
+          float diff = 1.0f;
+          const bool sane = !parameters.sanityCheck || Sketch::indexSanityCheck(ix, parameters.maxRatioDiff, diff);
+          if (!sane && b == 0) {
+            std::lock_guard<std::mutex> l(mu);
+            std::ostringstream m;                                       // the stream formatting of the per-split line
+            m << "ERROR :: SPLIT " << g << " chunk " << chunkNo << "'s ratio difference " << diff << " exceeds maximum thresholds.";
+            chunkSanity[g].push_back(m.str());
+          }
+          if (sane) {
+            bani_cgi_result *res = nullptr; uint64_t n = 0; bani_map_counters ctr;
+            const bani_qsketch *one = qsk;
+            check(bani_map_cgi_sketch(ctx, ix, &one, 1, &res, &n, &ctr), "bani_map_cgi_sketch");
+            for (uint64_t i = 0; i < n; i++)
+              local.push_back(cgi::CGI_Results{first + res[i].refGenomeId, res[i].qryGenomeId, res[i].countSeq, res[i].totalQueryFragments, res[i].identity});
+            bani_free(res);
+          }
+          ixOwner.reset();
+          check(bani_ctx_trim(ctx), "bani_ctx_trim");
+          first += taken;
+          chunkNo++;
+        }
+      }
+    };
+
     auto shardWork = [&](int g) {
       try {
         auto t1 = Clock::now();
         bani_ctx *ctx = ctxs[g];
+        // ---- chunk plan: does the shard's index fit next to the query sketches and the mapping working set?  A saved index
+        //      is one index per shard, so a run that loads one has one chunk.
+        std::vector<std::pair<int, int>> chunks(1, {0, (int)shards[g].size()}), blocks(1, {0, (int)parameters.querySequences.size()});
+        uint64_t indexBudget = 0;
+        if (!loading) {
+          const auto &qs = parameters.querySequences;
+          std::vector<uint64_t> qlen(qs.size()), rlen; std::vector<int32_t> rcont;
+          for (size_t q = 0; q < qs.size(); q++) for (const auto &c : genomes[pathId.at(qs[q])].contigs) qlen[q] += c.len;
+          for (int j : shards[g]) {
+            const auto &h = genomes[pathId.at(parameters.refSequences[j])];
+            uint64_t len = 0; for (const auto &c : h.contigs) len += c.len;
+            rlen.push_back(len); rcont.push_back((int32_t)h.contigs.size());
+          }
+          std::vector<int32_t> cEnd(std::max<size_t>(rlen.size(), 1)), bEnd(std::max<size_t>(qs.size(), 1));
+          int32_t nc = 0, nb = 0;
+          check(bani_ctx_plan_run(ctx, 0, 0, rlen.data(), rcont.data(), (int32_t)rlen.size(), qlen.data(), nullptr, (int32_t)qs.size(),
+                                  cEnd.data(), &nc, bEnd.data(), &nb, &indexBudget), "bani_ctx_plan_run");
+          if (nc > 0) { chunks.clear(); for (int32_t c = 0, a = 0; c < nc; a = cEnd[c], c++) chunks.push_back({a, cEnd[c]}); }
+          if (nb > 0) { blocks.clear(); for (int32_t c = 0, a = 0; c < nb; a = bEnd[c], c++) blocks.push_back({a, bEnd[c]}); }
+        }
         {
+          std::lock_guard<std::mutex> l(mu);
+          std::cerr << "INFO [GPU " << g << "], skch::main, reference chunks : " << chunks.size() << ", query blocks : " << blocks.size()
+                    << " (index budget " << indexBudget << " bytes)" << std::endl;
+        }
+        if (chunks.size() > 1 || blocks.size() > 1) {
+          if (parameters.visualize)
+            throw std::runtime_error("--visualize needs the reference shard of a GPU in one index, this run needs " + std::to_string(chunks.size()) +
+                                     " chunk(s) and " + std::to_string(blocks.size()) + " query block(s) on GPU " + std::to_string(g) + ": use more GPUs or fewer references");
+          if (!parameters.saveIndex.empty())
+            throw std::runtime_error("--saveIndex writes one index per GPU, this run needs " + std::to_string(chunks.size()) + " chunk(s) and " +
+                                     std::to_string(blocks.size()) + " query block(s) on GPU " + std::to_string(g) + ": use more GPUs or fewer references");
+          std::vector<cgi::CGI_Results> local;
+          chunkedShard(ctx, g, shards[g], chunks, blocks, indexBudget, local);
+          if (g == 0) std::cerr << "INFO [GPU 0], skch::main, Time spent sketching and mapping in chunks : "
+                                << std::chrono::duration<double>(Clock::now() - t1).count() << " sec" << std::endl;
+          cgi::correctRefGenomeIds(local, g, G, (int)parameters.refSequences.size(), parameters.blockPartition);
+          std::lock_guard<std::mutex> l(mu);
+          finalResults.insert(finalResults.end(), local.begin(), local.end());
+        } else {
           // genomes this device needs: its reference shard (unless loaded) and every query that has to be read, each file once
           std::vector<int> need; std::unordered_map<int, int> slot;
           auto want = [&](const std::string &path) { const int id = pathId.at(path); if (!slot.count(id)) { slot[id] = (int)need.size(); need.push_back(id); } return slot[id]; };
@@ -351,8 +453,10 @@ int main(int argc, char **argv)
     }
     if (!err.empty()) throw std::runtime_error(err);
     if (!parameters.saveIndex.empty()) writeMeta(parameters.saveIndex, parameters, G, savedContigNames);
-    for (int g = 0; g < G; g++)
+    for (int g = 0; g < G; g++) {
       if (!sanity[g]) std::cerr << "ERROR :: SPLIT " << g << "'s ratio difference " << ratioDiffs[g] << " exceeds maximum thresholds." << std::endl;
+      for (const auto &m : chunkSanity[g]) std::cerr << m << std::endl;
+    }
     // a query derived from the index has the length its reference twin has
     for (const auto &q : parameters.querySequences) if (!genomeLengths.count(q)) throw std::runtime_error("no length known for " + q);
 

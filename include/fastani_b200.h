@@ -126,7 +126,12 @@ BANI_API void *bani_ctx_stream(bani_ctx *ctx);
  * "event_bytes_per_piece" (0 = a quarter of device memory: a piece whose L2 event streams take more is mapped in halves),
  * "cgi_table_queries" (0 = as many as 3 GiB of bin table hold: queries per pass of the identity reduction),
  * "l2_fast" (1; 0 sends every L2 candidate to the exact kernel).  "count_paths" (default 0) turns on the branch counters
- * of bani_ctx_path_counts; with it off the mapping launches exactly the same kernels with the same work. */
+ * of bani_ctx_path_counts; with it off the mapping launches exactly the same kernels with the same work.
+ * Budgets of a run that builds its reference list in chunks (bani_ctx_plan_run; results never depend on them):
+ * "index_bytes_budget" (0 = derived from device memory: the build peak one chunk's index may take) and
+ * "query_sketch_budget" (0 = derived: a quarter of the free device memory; query sketches above it are mapped in blocks).
+ * Environment defaults: BANI_INDEX_BUDGET, BANI_QUERY_BUDGET (bytes, optionally with a K, M or G suffix, binary units); a
+ * value that is not a byte count makes bani_ctx_create fail with BANI_ERR_ARG. */
 BANI_API int  bani_ctx_set_flag(bani_ctx *ctx, const char *name, int64_t value);
 
 /* Which branches of the mapping path ran since the last call (counted only while the switch "count_paths" is on):
@@ -145,6 +150,14 @@ BANI_API int  bani_ctx_path_counts(bani_ctx *ctx, char (*names)[32], uint64_t *c
 BANI_API int  bani_ctx_profile_enable(bani_ctx *ctx, int on);
 BANI_API int  bani_ctx_profile_read(bani_ctx *ctx, char (*names)[32], double *ms, double *algo_bytes,
                                     int32_t *launches, int32_t n_max, int32_t *n);
+
+/* Device memory of the context's DEVICE as the caching allocator sees it (every context and index on that device counts):
+ * bytes handed out and not freed, bytes freed and kept for reuse, and the most bytes handed out at once since the previous
+ * call (read and reset).  bani_ctx_trim drops the context's scratch slots and returns every cached block of the device to
+ * the driver: blocks are cached by exact size, so a run that builds indexes of different sizes one after another calls
+ * it between them. */
+BANI_API int  bani_ctx_mem_stats(bani_ctx *ctx, uint64_t *live, uint64_t *cached, uint64_t *peak_live);
+BANI_API int  bani_ctx_trim(bani_ctx *ctx);
 
 /* Number of this library's own kernels launched on the context so far (CUB launches excluded). */
 BANI_API uint64_t bani_ctx_launch_count(const bani_ctx *ctx);
@@ -195,6 +208,60 @@ BANI_API int  bani_genome_decode(bani_ctx *ctx, const bani_genome *g, int32_t co
  * winSketch.hpp:75,167).  An empty list builds an empty index. */
 BANI_API int  bani_index_build(bani_ctx *ctx, bani_genome *const *refs, int32_t n_refs, bani_index **out);
 BANI_API void bani_index_destroy(bani_index *ix);
+/* The index of the longest prefix of refs whose build fits in max_bytes of device memory (bani_index_footprint with the
+ * exact record count of every genome, known after the sketch launch, and U bounded by it), at least one genome:
+ * *n_taken genomes, the index equal byte for byte to bani_index_build's of exactly those.  A first genome that does not
+ * fit alone gives BANI_ERR_LIMIT (never a failed allocation).  *peak_bytes (optional): the most device memory the call
+ * held above what was held on entry. */
+BANI_API int  bani_index_build_budget(bani_ctx *ctx, bani_genome *const *refs, int32_t n_refs, uint64_t max_bytes,
+                                      bani_index **out, int32_t *n_taken, uint64_t *peak_bytes);
+
+/* ---- chunked runs: footprint, budget and plan (host arithmetic, no device needed) ----------------------------------
+ * bani_index_footprint: peak device bytes of an index build of n_minimizers records (U <= n_unique_bound, n_contigs
+ * contigs, bitmap_bits validity bits, th/tw/ts staging for staging_cap records) and the bytes of the index it leaves.
+ * bani_map_working_set: the mapping working set bounded by the piece caps (max_hits_per_piece x 12 B of L1 staging, the L2
+ * event cap -- event_bytes_per_piece, 0 = a quarter of device_bytes -- and the 3 GiB bin table of the identity reduction).
+ * bani_run_working_set: the working set a run can reach, each term clamped by its cap: about query_hashes x n_refs hits
+ * (a query hash meets a reference genome about once), one L2 candidate per query fragment and reference genome, the bin
+ * table of ref_bases and n_queries -- megabytes for a run of a few genomes, the caps for a run of config 3's size.
+ * bani_index_budget: the build peak of the largest index (at the expected 2 / (w + 1) minimizers per base) for which
+ * max(build peak, resident index + working set) <= free_bytes - query_sketch_bytes: the build and the mapping are never
+ * alive at once.  bani_plan_chunks: cuts genomes (total length, contig count) into consecutive chunks, each the longest
+ * run whose expected build peak fits the budget and whose staging stays below 2^32 records; chunk c ends before genome
+ * chunk_end[c] (cap >= n).  A genome that alone exceeds the budget gives BANI_ERR_LIMIT naming it.
+ * bani_qsketch_bytes_estimate: export bytes of a genome's query sketch before it is built.
+ * bani_plan_run: the plan of one GPU's run -- reference chunks (chunk_end, cap >= n_refs) and query blocks (block_end,
+ * cap >= n_queries) -- from the free bytes, the device size, the piece caps and the budgets (0 = derived; the forced
+ * values of "index_bytes_budget" / "query_sketch_budget").  query_sketch_bytes (optional) are the sketches' export bytes,
+ * else they are estimated from query_len.  Query sketches above the query budget are mapped in blocks, unless that
+ * budget is derived and the run fits one index with every sketch resident.  The index budget leaves room for the largest
+ * block's sketches and the working set that block can reach (bani_run_working_set).  A derived budget that cannot hold a
+ * genome does not refuse the run: it is planned as one chunk and one block, on one index, as a run that fits; a forced one
+ * gives BANI_ERR_LIMIT naming the genome.  *index_budget_used (optional): the budget the chunks were cut with.
+ * bani_ctx_plan_run: the same with this context's free device memory (cudaMemGetInfo plus the cached blocks), size,
+ * switches and parameters; index_budget / query_budget override the switches when not 0. */
+BANI_API int  bani_index_footprint(uint64_t n_minimizers, uint64_t n_unique_bound, uint64_t n_contigs, uint64_t bitmap_bits,
+                                   uint64_t staging_cap, uint64_t *build_peak, uint64_t *resident);
+BANI_API int  bani_map_working_set(uint64_t device_bytes, int64_t max_hits_per_piece, int64_t event_bytes_per_piece, uint64_t *bytes);
+BANI_API int  bani_run_working_set(uint64_t device_bytes, int64_t max_hits_per_piece, int64_t event_bytes_per_piece,
+                                   uint64_t query_hashes, uint64_t query_fragments, int32_t n_queries, uint64_t ref_bases,
+                                   int32_t n_refs, int32_t window_size, int32_t frag_len, uint64_t *bytes);
+BANI_API int  bani_index_budget(uint64_t free_bytes, uint64_t query_sketch_bytes, uint64_t working_set, int32_t window_size,
+                                uint64_t *budget);
+BANI_API int  bani_plan_chunks(const uint64_t *genome_len, const int32_t *genome_contigs, int32_t n, int32_t k, int32_t w,
+                               uint64_t budget, int32_t *chunk_end, int32_t *n_chunks);
+BANI_API int  bani_qsketch_bytes_estimate(uint64_t len, int32_t w, int32_t frag_len, uint64_t *bytes);
+BANI_API int  bani_plan_run(uint64_t free_bytes, uint64_t device_bytes, int64_t max_hits_per_piece, int64_t event_bytes_per_piece,
+                            uint64_t index_budget, uint64_t query_budget, int32_t k, int32_t w, int32_t frag_len,
+                            const uint64_t *ref_len, const int32_t *ref_contigs, int32_t n_refs, const uint64_t *query_len,
+                            const uint64_t *query_sketch_bytes, int32_t n_queries, int32_t *chunk_end, int32_t *n_chunks,
+                            int32_t *block_end, int32_t *n_blocks, uint64_t *index_budget_used);
+BANI_API int  bani_ctx_plan_run(bani_ctx *ctx, uint64_t index_budget, uint64_t query_budget, const uint64_t *ref_len, const int32_t *ref_contigs, int32_t n_refs,
+                                const uint64_t *query_len, const uint64_t *query_sketch_bytes, int32_t n_queries,
+                                int32_t *chunk_end, int32_t *n_chunks, int32_t *block_end, int32_t *n_blocks,
+                                uint64_t *index_budget_used);
+/* "123", "64M", "2G" (binary units) -> bytes: how BANI_INDEX_BUDGET / BANI_QUERY_BUDGET are read. */
+BANI_API int  bani_parse_byte_count(const char *s, uint64_t *out);
 /* Totals needed by Sketch::sanityCheck (winSketch.hpp:298-318) and the log lines. */
 BANI_API int  bani_index_stats(const bani_index *ix, uint64_t *n_minimizers, uint64_t *n_unique,
                                uint64_t *total_len, uint64_t *n_contigs, uint64_t *n_genomes);
