@@ -25,6 +25,9 @@ MAPPING_DTYPE = np.dtype([
 MINIMIZER_DTYPE = np.dtype([("hash", "<u4"), ("seqId", "<i4"), ("wpos", "<i4")])
 CGI_DTYPE = np.dtype([("refGenomeId", "<i4"), ("qryGenomeId", "<i4"), ("countSeq", "<i4"),
                       ("totalQueryFragments", "<i4"), ("identity", "<f4")])
+# bani_frag_mapping: one 2-way mapping behind a CGI_DTYPE row (what a .visual line shows)
+FRAG_DTYPE = np.dtype([("qryGenomeId", "<i4"), ("querySeqId", "<i4"), ("refSeqId", "<i4"), ("refStartPos", "<i4"),
+                       ("identity", "<f4")])
 
 
 class BaniError(RuntimeError):
@@ -107,6 +110,7 @@ def load_library():
         "bani_qsketch_import": (C.c_int, [vp, vp, u64, P(vp)]),
         "bani_qsketch_merge": (C.c_int, [vp, P(vp), i32, P(vp)]),
         "bani_map_cgi_sketch": (C.c_int, [vp, vp, P(vp), i32, P(vp), P(u64), P(MapCounters)]),
+        "bani_map_cgi_sketch_frags": (C.c_int, [vp, vp, P(vp), i32, P(vp), P(u64), P(vp), P(u64), P(MapCounters)]),
         "bani_free": (None, [vp]),
         "bani_synth_genome": (C.c_int, [vp, u64, u32, u32, u32, i64, vp]),
         "bani_index_build_budget": (C.c_int, [vp, P(vp), i32, u64, P(vp), P(i32), P(u64)]),
@@ -138,7 +142,7 @@ EXPORTED_SYMBOLS = [
     "bani_index_destroy", "bani_index_stats", "bani_index_minimizers", "bani_index_save", "bani_index_load", "bani_index_contigs",
     "bani_qsketch_from_index", "bani_index_lookup", "bani_map_genome",
     "bani_map_cgi", "bani_free", "bani_synth_genome", "bani_qsketch_create", "bani_qsketch_destroy", "bani_qsketch_info",
-    "bani_qsketch_export", "bani_qsketch_import", "bani_qsketch_merge", "bani_map_cgi_sketch",
+    "bani_qsketch_export", "bani_qsketch_import", "bani_qsketch_merge", "bani_map_cgi_sketch", "bani_map_cgi_sketch_frags",
     "bani_index_build_budget", "bani_ctx_mem_stats", "bani_ctx_trim", "bani_ctx_plan_run", "bani_plan_run", "bani_run_working_set", "bani_index_footprint",
     "bani_map_working_set", "bani_index_budget", "bani_plan_chunks", "bani_qsketch_bytes_estimate", "bani_parse_byte_count"]
 
@@ -613,18 +617,30 @@ class QuerySketch:
             pass
 
 
-def compute_cgi_sketched(ctx, refSketch, query_sketches):
-    """compute_cgi for prebuilt QuerySketch objects; qryGenomeId = the query_ids the sketches were built with."""
+def _take_records(lib, ptr, n, dtype):
+    if not n.value:
+        return np.empty(0, dtype)
+    out = _records_from(ptr.value, n.value, dtype)
+    lib.bani_free(ptr)
+    return out
+
+
+def compute_cgi_sketched(ctx, refSketch, query_sketches, fragments=False):
+    """compute_cgi for prebuilt QuerySketch objects; qryGenomeId = the query_ids the sketches were built with.
+    Returns (results[CGI_DTYPE], MapCounters).  fragments=True (bani_map_cgi_sketch_frags) returns
+    (results, MapCounters, frags[FRAG_DTYPE]): the same results and the 2-way mappings behind them, ordered by
+    (sketch, query, refSeqId, position bin); report.visual_lines writes them as .visual lines."""
     qs = list(query_sketches)
     arr = (C.c_void_p * max(len(qs), 1))(*[q.h for q in qs])
     res = C.c_void_p(); n = C.c_uint64(); ctr = MapCounters()
-    _check(ctx.lib.bani_map_cgi_sketch(ctx.h, refSketch.h, arr, len(qs), C.byref(res), C.byref(n), C.byref(ctr)))
-    if n.value:
-        out = _records_from(res.value, n.value, CGI_DTYPE)
-        ctx.lib.bani_free(res)
-    else:
-        out = np.empty(0, CGI_DTYPE)
-    return out, ctr
+    if not fragments:
+        _check(ctx.lib.bani_map_cgi_sketch(ctx.h, refSketch.h, arr, len(qs), C.byref(res), C.byref(n), C.byref(ctr)))
+        return _take_records(ctx.lib, res, n, CGI_DTYPE), ctr
+    fr = C.c_void_p(); nf = C.c_uint64()
+    _check(ctx.lib.bani_map_cgi_sketch_frags(ctx.h, refSketch.h, arr, len(qs), C.byref(res), C.byref(n), C.byref(fr), C.byref(nf),
+                                             C.byref(ctr)))
+    out = _take_records(ctx.lib, res, n, CGI_DTYPE)
+    return out, ctr, _take_records(ctx.lib, fr, nf, FRAG_DTYPE)
 
 
 # ---------------------------------------------------------------------------------------- chunked runs

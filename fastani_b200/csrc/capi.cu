@@ -28,6 +28,26 @@ using namespace bani;
   catch (const std::bad_alloc &) { bani::set_last_error("host allocation failed"); return BANI_ERR_NOMEM; } \
   catch (const std::exception &e) { bani::set_last_error(e.what()); return BANI_ERR_INTERNAL; }
 
+// a malloc'ed copy of v (nullptr when empty), for the caller to bani_free
+template <typename T>
+static T *host_copy(const std::vector<T> &v)
+{
+  if (v.empty()) return nullptr;
+  T *p = (T *)malloc(sizeof(T) * v.size());
+  if (!p) fail(BANI_ERR_NOMEM, "host allocation failed");
+  memcpy(p, v.data(), sizeof(T) * v.size());
+  return p;
+}
+
+static void map_cgi_sketch(bani_ctx *ctx, const bani_index *ix, const bani_qsketch *const *sketches, int32_t n_sketches, bool wantFrags,
+                           MapOutput &mo)
+{
+  BANI_CUDA(cudaSetDevice(ctx->c.device));
+  std::vector<const QSketch *> qs(n_sketches);
+  for (int i = 0; i < n_sketches; i++) { if (!sketches[i] || !sketches[i]->qs) fail(BANI_ERR_ARG, "null query sketch"); qs[i] = sketches[i]->qs; }
+  qsketch_map(&ctx->c, ix->ix, qs.data(), n_sketches, false, true, mo, wantFrags);
+}
+
 extern "C" {
 
 const char *bani_last_error(void) { return g_err.c_str(); }
@@ -765,18 +785,29 @@ int bani_map_cgi_sketch(bani_ctx *ctx, const bani_index *ix, const bani_qsketch 
 {
   BANI_TRY
   if (!ctx || !ix || !ix->ix || n_sketches < 0 || (n_sketches && !sketches) || !results || !n_results) fail(BANI_ERR_ARG, "null argument");
-  BANI_CUDA(cudaSetDevice(ctx->c.device));
-  std::vector<const QSketch *> qs(n_sketches);
-  for (int i = 0; i < n_sketches; i++) { if (!sketches[i] || !sketches[i]->qs) fail(BANI_ERR_ARG, "null query sketch"); qs[i] = sketches[i]->qs; }
   MapOutput mo;
-  qsketch_map(&ctx->c, ix->ix, qs.data(), n_sketches, false, true, mo);
+  map_cgi_sketch(ctx, ix, sketches, n_sketches, false, mo);
+  *results = host_copy(mo.cgi);
   *n_results = mo.cgi.size();
-  *results = nullptr;
-  if (!mo.cgi.empty()) {
-    *results = (bani_cgi_result *)malloc(sizeof(bani_cgi_result) * mo.cgi.size());
-    if (!*results) fail(BANI_ERR_NOMEM, "host allocation failed");
-    memcpy(*results, mo.cgi.data(), sizeof(bani_cgi_result) * mo.cgi.size());
-  }
+  if (counters) *counters = mo.ctr;
+  return BANI_OK;
+  BANI_CATCH
+}
+
+int bani_map_cgi_sketch_frags(bani_ctx *ctx, const bani_index *ix, const bani_qsketch *const *sketches, int32_t n_sketches,
+                              bani_cgi_result **results, uint64_t *n_results, bani_frag_mapping **frags, uint64_t *n_frags,
+                              bani_map_counters *counters)
+{
+  BANI_TRY
+  if (!ctx || !ix || !ix->ix || n_sketches < 0 || (n_sketches && !sketches) || !results || !n_results || !frags || !n_frags)
+    fail(BANI_ERR_ARG, "null argument");
+  MapOutput mo;
+  map_cgi_sketch(ctx, ix, sketches, n_sketches, true, mo);
+  std::unique_ptr<bani_cgi_result, void (*)(void *)> res(host_copy(mo.cgi), free);
+  *frags = host_copy(mo.frags);
+  *n_frags = mo.frags.size();
+  *results = res.release();
+  *n_results = mo.cgi.size();
   if (counters) *counters = mo.ctr;
   return BANI_OK;
   BANI_CATCH

@@ -369,6 +369,7 @@ Index *index_load(Ctx *ctx, const char *path);
 struct MapOutput {
   std::vector<bani_mapping> rows;               // when wantRows
   std::vector<bani_cgi_result> cgi;             // when wantCgi
+  std::vector<bani_frag_mapping> frags;         // when wantFrags: the 2-way mappings behind cgi
   std::vector<uint64_t> totalQueryFragments;    // per query
   bani_map_counters ctr{};
 };
@@ -380,8 +381,9 @@ uint64_t qsketch_export_bytes(const QSketch *qs);
 void qsketch_export(Ctx *ctx, const QSketch *qs, void *devBuf, uint64_t cap);
 QSketch *qsketch_import(Ctx *ctx, const void *devBuf, uint64_t bytes);
 QSketch *qsketch_merge(Ctx *ctx, const QSketch *const *sketches, int32_t n);
+// wantFrags (implies wantCgi): the identity reduction also records which fragment won each bin (out.frags)
 void qsketch_map(Ctx *ctx, const Index *ix, const QSketch *const *sketches, int32_t nSketches,
-                 bool wantRows, bool wantCgi, MapOutput &out);
+                 bool wantRows, bool wantCgi, MapOutput &out, bool wantFrags = false);
 
 // hits.cu : per-fragment gather + shared-memory sort + L1 candidate regions
 static constexpr unsigned long long FRAG_L1_MAX = 8192;   // hits per fragment handled inside one CTA
@@ -420,6 +422,9 @@ void   cub_sort_pairs_u32(void *temp, size_t tempBytes, const uint32_t *kin, uin
 size_t cub_sort_keys_u64_temp(size_t n);
 void   cub_sort_keys_u64(void *temp, size_t tempBytes, const uint64_t *kin, uint64_t *kout, size_t n,
                          int beginBit, int endBit, cudaStream_t s);
+size_t cub_sort_pairs_u64_u32_temp(size_t n);
+void   cub_sort_pairs_u64_u32(void *temp, size_t tempBytes, const uint64_t *kin, uint64_t *kout,
+                              const uint32_t *vin, uint32_t *vout, size_t n, int endBit, cudaStream_t s);
 size_t cub_scan_u32_temp(size_t n);
 void   cub_exclusive_sum_u32(void *temp, size_t tempBytes, const uint32_t *in, uint32_t *out, size_t n, cudaStream_t s);
 size_t cub_scan_u64_temp(size_t n);

@@ -30,6 +30,18 @@ void cub_sort_keys_u64(void *temp, size_t tempBytes, const uint64_t *kin, uint64
 {
   BANI_CUDA(cub::DeviceRadixSort::SortKeys(temp, tempBytes, kin, kout, n, beginBit, endBit, s));
 }
+size_t cub_sort_pairs_u64_u32_temp(size_t n)
+{
+  size_t b = 0;
+  cub::DeviceRadixSort::SortPairs(nullptr, b, (const uint64_t *)nullptr, (uint64_t *)nullptr,
+                                  (const uint32_t *)nullptr, (uint32_t *)nullptr, n);
+  return b;
+}
+void cub_sort_pairs_u64_u32(void *temp, size_t tempBytes, const uint64_t *kin, uint64_t *kout,
+                            const uint32_t *vin, uint32_t *vout, size_t n, int endBit, cudaStream_t s)
+{
+  BANI_CUDA(cub::DeviceRadixSort::SortPairs(temp, tempBytes, kin, kout, vin, vout, n, 0, endBit, s));
+}
 size_t cub_scan_u32_temp(size_t n)
 {
   size_t b = 0;

@@ -808,7 +808,23 @@ struct CgiArgs {
 };
 
 // 1-way: best row of each (fragment, genome) by (identity, refSeqId, refStartPos) (cgid_types.hpp:31-39,
-// computeCoreIdentity.hpp:214-231); 2-way: best identity per (ref contig, position bin) (:237-254)
+// computeCoreIdentity.hpp:214-231): true if no other row of fragment f (row i, identity id) on genome g beats row i
+__device__ __forceinline__ bool cgi_one_way_winner(const CgiArgs &a, uint32_t i, int f, int g, float id)
+{
+  // rows of a fragment are contiguous and ordered by (refSeqId, refStartPos): a later row wins ties
+  for (uint32_t j = i + 1; j < a.R && a.rFrag[j] == f && a.contigGenome[a.rows[j].refSeqId] == g; j++)
+    if (a.rows[j].nucIdentity >= id) return false;
+  for (uint32_t j = i; j-- > 0 && a.rFrag[j] == f && a.contigGenome[a.rows[j].refSeqId] == g;)
+    if (a.rows[j].nucIdentity > id) return false;
+  return true;
+}
+
+__device__ __forceinline__ unsigned long long cgi_bin(const CgiArgs &a, const bani_mapping &r)
+{
+  return a.contigBinOff[r.refSeqId] + (uint32_t)(r.refStartPos / (a.fragLen - 20));
+}
+
+// 2-way: best identity per (ref contig, position bin) (:237-254)
 __global__ void cgi_scatter_kernel(const CgiArgs a)
 {
   uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -818,20 +834,73 @@ __global__ void cgi_scatter_kernel(const CgiArgs a)
   if (q < a.qLo || q >= a.qHi) return;
   const bani_mapping r = a.rows[i];
   const int g = a.contigGenome[r.refSeqId];
-  // rows of a fragment are contiguous and ordered by (refSeqId, refStartPos): a later row wins ties
-  for (uint32_t j = i + 1; j < a.R && a.rFrag[j] == f && a.contigGenome[a.rows[j].refSeqId] == g; j++)
-    if (a.rows[j].nucIdentity >= r.nucIdentity) return;
-  for (uint32_t j = i; j-- > 0 && a.rFrag[j] == f && a.contigGenome[a.rows[j].refSeqId] == g;)
-    if (a.rows[j].nucIdentity > r.nucIdentity) return;
-  const unsigned long long bin = a.contigBinOff[r.refSeqId] + (uint32_t)(r.refStartPos / (a.fragLen - 20));
-  atomicMax(a.table + (unsigned long long)(q - a.qLo) * a.totalBins + bin, __float_as_uint(r.nucIdentity));
+  if (!cgi_one_way_winner(a, i, f, g, r.nucIdentity)) return;
+  atomicMax(a.table + (unsigned long long)(q - a.qLo) * a.totalBins + cgi_bin(a, r), __float_as_uint(r.nucIdentity));
   a.touched[(size_t)(q - a.qLo) * a.nGenomes + g] = 1;
 }
 
+// Fragment-row mode of stage H (bani_map_cgi_sketch_frags): each bin holds the 64-bit key (identity bits << 32 | querySeqId)
+// of its winner.  Every row of one table row and bin has the same query and genome, and positive floats order as their
+// bits, so the 64-bit maximum is the best identity and, among equal identities, the largest querySeqId: the last element
+// of computeCGI's stable sort over the 1-way list, which is ordered by (genome, querySeqId) (computeCoreIdentity.hpp:237-254).
+struct CgiFragArgs {
+  unsigned long long *table;           // [querySlot - qLo][totalBins] keys, 0 = empty
+  uint8_t *win;                        // per row: 1-way winner of this pass
+  unsigned long long *key; uint32_t *row; uint32_t *count;   // emitted 2-way winners: (query slot << 32 | global bin), row
+};
+
+__device__ __forceinline__ unsigned long long cgi_frag_key(const bani_mapping &r)
+{
+  return ((unsigned long long)__float_as_uint(r.nucIdentity) << 32) | (uint32_t)r.querySeqId;
+}
+
+__global__ void cgi_scatter_frag_kernel(const CgiArgs a, const CgiFragArgs f)
+{
+  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= a.R) return;
+  const int fr = a.rFrag[i];
+  const int q = a.fragQuery[fr];
+  const bani_mapping r = a.rows[i];
+  const int g = a.contigGenome[r.refSeqId];
+  const bool w = q >= a.qLo && q < a.qHi && cgi_one_way_winner(a, i, fr, g, r.nucIdentity);
+  f.win[i] = w;
+  if (!w) return;
+  atomicMax(f.table + (unsigned long long)(q - a.qLo) * a.totalBins + cgi_bin(a, r), cgi_frag_key(r));
+  a.touched[(size_t)(q - a.qLo) * a.nGenomes + g] = 1;
+}
+
+// the 1-way winners that hold their bin's key: one per non-empty bin, appended in any order (sorted afterwards)
+__global__ void cgi_emit_kernel(const CgiArgs a, const CgiFragArgs f)
+{
+  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= a.R || !f.win[i]) return;
+  const bani_mapping r = a.rows[i];
+  const int q = a.fragQuery[a.rFrag[i]];
+  const unsigned long long bin = cgi_bin(a, r);
+  if (f.table[(unsigned long long)(q - a.qLo) * a.totalBins + bin] != cgi_frag_key(r)) return;
+  const uint32_t o = atomicAdd(f.count, 1u);
+  f.key[o] = ((unsigned long long)q << 32) | bin;
+  f.row[o] = i;
+}
+
+// sorted (query slot, bin) keys -> records; qryGenomeId holds the piece-local query slot until the host maps it
+__global__ void cgi_frag_gather_kernel(const bani_mapping *rows, const unsigned long long *key, const uint32_t *row, uint32_t n,
+                                       bani_frag_mapping *out)
+{
+  uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  const bani_mapping r = rows[row[j]];
+  bani_frag_mapping m;
+  m.qryGenomeId = (int32_t)(key[j] >> 32); m.querySeqId = r.querySeqId; m.refSeqId = r.refSeqId; m.refStartPos = r.refStartPos;
+  m.identity = r.nucIdentity;
+  out[j] = m;
+}
+
 // ordered float32 sum over the bins of one (query, genome) pair (computeCoreIdentity.hpp:267-297);
-// clears what it read so the table is all-zero again for the next chunk
-__global__ void cgi_sum_kernel(uint32_t *table, uint8_t *touched, const uint32_t *contigBinOff, const int32_t *genomeContigEnd,
-                               unsigned long long totalBins, int nGenomes, int nQ, int32_t *oCount, float *oIdent)
+// clears what it read so the table is all-zero again for the next chunk.  The identity is the high word of a 64-bit key.
+template <typename T>
+__device__ __forceinline__ void cgi_sum_pair(T *table, uint8_t *touched, const uint32_t *contigBinOff, const int32_t *genomeContigEnd,
+                                             unsigned long long totalBins, int nGenomes, int nQ, int32_t *oCount, float *oIdent)
 {
   uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (uint32_t)nQ * (uint32_t)nGenomes) return;
@@ -840,10 +909,25 @@ __global__ void cgi_sum_kernel(uint32_t *table, uint8_t *touched, const uint32_t
   if (touched[i]) {
     touched[i] = 0;
     const uint32_t b0 = contigBinOff[g ? genomeContigEnd[g - 1] : 0], b1 = contigBinOff[genomeContigEnd[g]];
-    uint32_t *row = table + (unsigned long long)q * totalBins;
-    for (uint32_t b = b0; b < b1; b++) { uint32_t v = row[b]; if (v) { sum += __uint_as_float(v); cnt++; row[b] = 0; } }
+    T *row = table + (unsigned long long)q * totalBins;
+    for (uint32_t b = b0; b < b1; b++) {
+      const T v = row[b];
+      if (v) { sum += __uint_as_float((uint32_t)(v >> (8 * sizeof(T) - 32))); cnt++; row[b] = 0; }
+    }
   }
   oCount[i] = cnt; oIdent[i] = cnt ? sum / cnt : 0.0f;
+}
+
+__global__ void cgi_sum_kernel(uint32_t *table, uint8_t *touched, const uint32_t *contigBinOff, const int32_t *genomeContigEnd,
+                               unsigned long long totalBins, int nGenomes, int nQ, int32_t *oCount, float *oIdent)
+{
+  cgi_sum_pair(table, touched, contigBinOff, genomeContigEnd, totalBins, nGenomes, nQ, oCount, oIdent);
+}
+
+__global__ void cgi_sum_frag_kernel(unsigned long long *table, uint8_t *touched, const uint32_t *contigBinOff, const int32_t *genomeContigEnd,
+                                    unsigned long long totalBins, int nGenomes, int nQ, int32_t *oCount, float *oIdent)
+{
+  cgi_sum_pair(table, touched, contigBinOff, genomeContigEnd, totalBins, nGenomes, nQ, oCount, oIdent);
 }
 
 // ------------------------------------------------------------------ host orchestration
@@ -1413,9 +1497,10 @@ void map_queries(Ctx *ctx, const Index *ix, const Genome *const *queries, int32_
 }
 
 void qsketch_map(Ctx *ctx, const Index *ix, const QSketch *const *sketches, int32_t nSketches,
-                 bool wantRows, bool wantCgi, MapOutput &out)
+                 bool wantRows, bool wantCgi, MapOutput &out, bool wantFrags)
 {
   cudaStream_t st = ctx->stream;
+  wantCgi = wantCgi || wantFrags;
   const int k = ctx->prm.kmer_size, w = ctx->prm.window_size, fragLen = ctx->prm.frag_len;
   const float pid = ctx->prm.perc_identity;
   if (ix->device != ctx->device) fail(BANI_ERR_ARG, "index lives on another device");
@@ -1426,15 +1511,16 @@ void qsketch_map(Ctx *ctx, const Index *ix, const QSketch *const *sketches, int3
   out.ctr = bani_map_counters{};
   const int nG = ix->nGenomes;
 
-  // the 2-way table holds a bounded number of queries at a time
+  // the 2-way table holds a bounded number of queries at a time (4-byte bins, 8-byte keys in the fragment-row mode)
   uint64_t qMaxByTable = 1u << 30;
-  if (wantCgi && ix->totalBins) qMaxByTable = std::max<uint64_t>(1, ((uint64_t)3 << 30) / (4 * ix->totalBins));
+  const uint64_t binBytes = wantFrags ? 8 : 4;
+  if (wantCgi && ix->totalBins) qMaxByTable = std::max<uint64_t>(1, ((uint64_t)3 << 30) / (binBytes * ix->totalBins));
   if (ctx->flags.cgiTableQueries > 0) qMaxByTable = std::min<uint64_t>(qMaxByTable, (uint64_t)ctx->flags.cgiTableQueries);
   // a piece whose L2 event streams would take more is mapped in halves
   const double evLimit = ctx->flags.eventBytesPerPiece > 0 ? (double)ctx->flags.eventBytesPerPiece : 0.25 * (double)ctx->memTotal;
   const bool countPaths = ctx->flags.countPaths != 0;
 
-  DevBuf<uint32_t> table; DevBuf<uint8_t> touched; DevBuf<int32_t> d_gce;
+  DevBuf<uint32_t> table; DevBuf<unsigned long long> table64; DevBuf<uint8_t> touched; DevBuf<int32_t> d_gce;
   uint64_t tableQ = 0;
   if (wantCgi) {
     d_gce.alloc(std::max(nG, 1), st);
@@ -1475,6 +1561,7 @@ void qsketch_map(Ctx *ctx, const Index *ix, const QSketch *const *sketches, int3
     View<int32_t> d_fragSeqId; d_fragSeqId.p = pc.fragSeqId.p; d_fragSeqId.n = F;
 
     std::vector<int32_t> hCount; std::vector<float> hIdent;
+    std::vector<bani_frag_mapping> hFrags;
     if (wantCgi) { hCount.assign((size_t)nQc * nG, 0); hIdent.assign((size_t)nQc * nG, 0.f); }
 
     ctx->mark("piece: begin");
@@ -1744,8 +1831,11 @@ void qsketch_map(Ctx *ctx, const Index *ix, const QSketch *const *sketches, int3
                 const uint64_t needQ = std::min<uint64_t>(qMaxByTable, std::max<uint64_t>(nQc, 1));
                 if (needQ > tableQ) {
                   tableQ = needQ;
-                  table.alloc((size_t)tableQ * ix->totalBins, st); touched.alloc((size_t)tableQ * std::max(nG, 1), st);
-                  BANI_CUDA(cudaMemsetAsync(table.p, 0, table.bytes(), st));
+                  if (wantFrags) table64.alloc((size_t)tableQ * ix->totalBins, st);
+                  else table.alloc((size_t)tableQ * ix->totalBins, st);
+                  touched.alloc((size_t)tableQ * std::max(nG, 1), st);
+                  if (wantFrags) BANI_CUDA(cudaMemsetAsync(table64.p, 0, table64.bytes(), st));
+                  else BANI_CUDA(cudaMemsetAsync(table.p, 0, table.bytes(), st));
                   BANI_CUDA(cudaMemsetAsync(touched.p, 0, touched.bytes(), st));
                 }
                 CgiArgs ca; ca.rows = rows.p; ca.rFrag = rFrag.p; ca.R = R; ca.fragQuery = d_fragQuery.p;
@@ -1753,7 +1843,8 @@ void qsketch_map(Ctx *ctx, const Index *ix, const QSketch *const *sketches, int3
                 ca.totalBins = ix->totalBins; ca.nGenomes = nG; ca.table = table.p; ca.touched = touched.p;
                 BANI_SCRATCH(int32_t, oCount, (size_t)nQc * nG);
                 DevBuf<float> oIdent((size_t)nQc * nG, st);
-                { Stage sg(ctx, "cgi", 48.0 * R);
+                if (!wantFrags) {
+                  Stage sg(ctx, "cgi", 48.0 * R);
                   for (int qa = 0; qa < nQc; qa += (int)tableQ) {
                     const int nPass = std::min<int>((int)tableQ, nQc - qa);
                     ca.qLo = qa; ca.qHi = qa + nPass;
@@ -1762,7 +1853,45 @@ void qsketch_map(Ctx *ctx, const Index *ix, const QSketch *const *sketches, int3
                     cgi_sum_kernel<<<nblk((uint64_t)nPass * nG), 256, 0, st>>>(table.p, touched.p, ix->contigBinOff.p, d_gce.p,
                                                                              ix->totalBins, nG, nPass, oCount.p + (size_t)qa * nG, oIdent.p + (size_t)qa * nG);
                     ctx->launches++;
-                  } }
+                  }
+                } else {
+                  // fragment-row mode: scatter 64-bit keys, emit each bin's winning row before the sum clears the bin, then
+                  // sort the piece's winners by (query slot, global bin) -- unique keys, so the order is deterministic
+                  BANI_SCRATCH(uint8_t, win, R);
+                  BANI_SCRATCH(unsigned long long, emKey, R);
+                  BANI_SCRATCH(unsigned long long, emKeySorted, R);
+                  BANI_SCRATCH(uint32_t, emRow, R);
+                  BANI_SCRATCH(uint32_t, emRowSorted, R);
+                  BANI_SCRATCH(uint32_t, emCount, 1);
+                  BANI_CUDA(cudaMemsetAsync(emCount.p, 0, 4, st));
+                  CgiFragArgs fa; fa.table = table64.p; fa.win = win.p; fa.key = emKey.p; fa.row = emRow.p; fa.count = emCount.p;
+                  Stage sg(ctx, "cgi_frags", 64.0 * R);
+                  for (int qa = 0; qa < nQc; qa += (int)tableQ) {
+                    const int nPass = std::min<int>((int)tableQ, nQc - qa);
+                    ca.qLo = qa; ca.qHi = qa + nPass;
+                    cgi_scatter_frag_kernel<<<nblk(R), 256, 0, st>>>(ca, fa);
+                    ctx->launches++; pp[P_CGI_PASSES]++;
+                    cgi_emit_kernel<<<nblk(R), 256, 0, st>>>(ca, fa);
+                    ctx->launches++;
+                    cgi_sum_frag_kernel<<<nblk((uint64_t)nPass * nG), 256, 0, st>>>(table64.p, touched.p, ix->contigBinOff.p, d_gce.p,
+                                                                                  ix->totalBins, nG, nPass, oCount.p + (size_t)qa * nG, oIdent.p + (size_t)qa * nG);
+                    ctx->launches++;
+                  }
+                  uint32_t nEm = 0;
+                  BANI_CUDA(cudaMemcpyAsync(&nEm, emCount.p, 4, cudaMemcpyDeviceToHost, st));
+                  BANI_CUDA(cudaStreamSynchronize(st));
+                  if (nEm > 0) {
+                    int qBits = 0; while ((1 << qBits) < nQc) qBits++;
+                    { size_t tb = cub_sort_pairs_u64_u32_temp(nEm);
+                      BANI_SCRATCH(uint8_t, tmp, tb);
+                      cub_sort_pairs_u64_u32(tmp.p, tb, (const uint64_t *)emKey.p, (uint64_t *)emKeySorted.p, emRow.p, emRowSorted.p, nEm, 32 + qBits, st); }
+                    BANI_SCRATCH(bani_frag_mapping, dFrags, nEm);
+                    cgi_frag_gather_kernel<<<nblk(nEm), 256, 0, st>>>(rows.p, emKeySorted.p, emRowSorted.p, nEm, dFrags.p);
+                    ctx->launches++;
+                    hFrags.resize(nEm);
+                    BANI_CUDA(cudaMemcpyAsync(hFrags.data(), dFrags.p, sizeof(bani_frag_mapping) * (size_t)nEm, cudaMemcpyDeviceToHost, st));
+                  }
+                }
                 ctx->mark("piece: cgi launched");
                 BANI_CUDA(cudaMemcpyAsync(hCount.data(), oCount.p, 4 * (size_t)nQc * nG, cudaMemcpyDeviceToHost, st));
                 BANI_CUDA(cudaMemcpyAsync(hIdent.data(), oIdent.p, 4 * (size_t)nQc * nG, cudaMemcpyDeviceToHost, st));
@@ -1784,6 +1913,10 @@ void qsketch_map(Ctx *ctx, const Index *ix, const QSketch *const *sketches, int3
     }
     if (wantCgi && !split) {
       append_cgi_rows(hCount.data(), hIdent.data(), nQc, nG, qs->queryId.data() + q0, qs->totalFragments.data() + q0, out.cgi);
+    }
+    if (wantFrags && !split) {
+      for (auto &m : hFrags) m.qryGenomeId = qs->queryId[q0 + m.qryGenomeId];
+      out.frags.insert(out.frags.end(), hFrags.begin(), hFrags.end());
     }
     ctx->mark("piece: rows assembled");
    }

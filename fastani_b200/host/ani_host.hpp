@@ -4,8 +4,8 @@
 //   skch::Parameters        src/map/include/map_parameters.hpp:22-41
 //   skch::Sketch            src/map/include/winSketch.hpp:43-343      (constructor = HP1, on the GPU)
 //   skch::Map               src/map/include/computeMap.hpp:35-560     (constructor = HP2, on the GPU)
-//   cgi::computeCGI ...     src/cgi/include/computeCoreIdentity.hpp   (host restatement, used for --visualize;
-//                                                                      the batch path uses the fused device reduction)
+//   cgi::computeCGI ...     src/cgi/include/computeCoreIdentity.hpp   (host restatement, kept for comparison behind
+//                                                                      BANI_CLI_HOST_CGI=1; the CLI uses the fused device reduction)
 //   cgi::outputCGI / outputPhylip / outputVisualizationFile / splitReferenceGenomes / correctRefGenomeIds
 //
 // Nothing here computes minimizers, hashes or identities on the CPU: Sketch and Map only hold handles of the
@@ -221,6 +221,15 @@ class Sketch {
 };
 
 // ---------------------------------------------------------------------------------------- Map (HP2)
+// computeMap.hpp:138-167: the Map::metadata lengths of one query contig (entry i of a genome belongs to querySeqId i): a
+// contig too short to map is one entry; any other gives len / fragLen fragments, the last one extended by len % fragLen
+inline void appendFragmentLengths(const Parameters &p, offset_t len, std::vector<offset_t> &out)
+{
+  if (len < p.windowSize || len < p.kmerSize || len < p.minReadLength) { out.push_back(len); return; }
+  const int fc = len / p.minReadLength;
+  for (int i = 0; i < fc; i++) out.push_back(i != fc - 1 ? p.minReadLength : p.minReadLength + (len % p.minReadLength));
+}
+
 class Map {
  public:
   std::vector<ContigInfo> metadata;                       // computeMap.hpp:84: filled only with --visualize
@@ -235,12 +244,11 @@ class Map {
     if (f) for (uint64_t i = 0; i < n; i++) f(rows[i]);
     bani_free(rows);
     if (p.visualize) {                                    // computeMap.hpp:138-167
+      std::vector<offset_t> lens;
       for (const auto &c : query.host->contigs) {
-        const offset_t len = (offset_t)c.len;
-        if (len < p.windowSize || len < p.kmerSize || len < p.minReadLength) { metadata.push_back(ContigInfo{c.name, len}); continue; }
-        const int fc = len / p.minReadLength;
-        for (int i = 0; i < fc; i++)
-          metadata.push_back(ContigInfo{c.name, i != fc - 1 ? p.minReadLength : p.minReadLength + (len % p.minReadLength)});
+        lens.clear();
+        appendFragmentLengths(p, (offset_t)c.len, lens);
+        for (offset_t l : lens) metadata.push_back(ContigInfo{c.name, l});
       }
     }
   }
@@ -293,6 +301,34 @@ inline void outputVisualizationFile(const skch::Parameters &parameters, const st
             << "\t" << e.queryStartPos + parameters.minReadLength - 1 + queryOffsetAdder[e.querySeqId]
             << "\t" << e.refStartPos + refOffsetAdder[e.refSequenceId]
             << "\t" << e.refStartPos + parameters.minReadLength - 1 + refOffsetAdder[e.refSequenceId]
+            << "\tNA\tNA\n";
+  }
+}
+
+// prefix sums of lengths: offset of entry i in the concatenation of entries 0 .. i-1
+inline std::vector<int64_t> offsetAdder(const std::vector<skch::offset_t> &lens)
+{
+  std::vector<int64_t> off(lens.size() + 1, 0);
+  for (size_t i = 0; i < lens.size(); i++) off[i + 1] = off[i] + lens[i];
+  return off;
+}
+
+// outputVisualizationFile for the 2-way mappings of one query from the device reduction (bani_map_cgi_sketch_frags).
+// queryOffsetAdder: offsetAdder of the query's Map::metadata lengths; refOffsetAdder: that of refSketch.metadata.
+inline void outputVisualizationFile(const skch::Parameters &parameters, const bani_frag_mapping *frags, size_t n,
+                                    const std::vector<int64_t> &queryOffsetAdder, const std::vector<int64_t> &refOffsetAdder,
+                                    const skch::Sketch &refSketch, const std::string &queryName,
+                                    const std::vector<std::string> &shardRefNames, std::ostream &outstrm)
+{
+  const auto &sbf = refSketch.sequencesByFileInfo;
+  for (size_t i = 0; i < n; i++) {
+    const bani_frag_mapping &e = frags[i];
+    const size_t g = std::upper_bound(sbf.begin(), sbf.end(), e.refSeqId) - sbf.begin();   // :29-41
+    outstrm << queryName << "\t" << shardRefNames[g] << "\t" << e.identity << "\tNA\tNA\tNA"
+            << "\t" << queryOffsetAdder[e.querySeqId]
+            << "\t" << parameters.minReadLength - 1 + queryOffsetAdder[e.querySeqId]
+            << "\t" << e.refStartPos + refOffsetAdder[e.refSeqId]
+            << "\t" << e.refStartPos + parameters.minReadLength - 1 + refOffsetAdder[e.refSeqId]
             << "\tNA\tNA\n";
   }
 }

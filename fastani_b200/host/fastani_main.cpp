@@ -10,8 +10,10 @@
 //     the same pass (the reference reads each file again in computeGenomeLengths, computeCoreIdentity.hpp:48-92)
 //   * --saveIndex / --loadIndex: the on-disk sketch cache the reference lacks (its only answer to repeated runs is
 //     scripts/splitDatabase.sh + README.md:104-106); parameters (k, fragLen, window) are stored and a mismatch is refused
-//   * without --visualize the per-pair reduction runs on the device (bani_map_cgi); with it, the mapping rows come
-//     back and cgi::computeCGI runs on the host because the .visual file needs the surviving rows themselves
+//   * the per-pair reduction runs on the device for every query of a GPU at once (bani_map_cgi_sketch); with --visualize
+//     it also returns the 2-way fragment mappings the .visual file is written from (bani_map_cgi_sketch_frags).
+//     BANI_CLI_HOST_CGI=1 (a test switch) instead maps one query at a time, copies its mapping rows back and runs
+//     cgi::computeCGI on the host, so that both paths can be compared on the same inputs
 #include <atomic>
 #include <chrono>
 #include <cstdlib>
@@ -228,11 +230,13 @@ int main(int argc, char **argv)
       ctxThreads.emplace_back([&, g]() { bani_params cp = parameters.c(); if (bani_ctx_create(g, &cp, &ctxs[g]) != BANI_OK) ctxErr[g] = bani_last_error(); });
 
     // ---- ingest: every distinct file once, in parallel.  With a loaded index no reference file is read, and (one
-    //      shard, no --visualize) neither is a query that is a genome of the index: its sketch is derived from the index
+    //      shard) neither is a query that is a genome of the index: its sketch is derived from the index
     auto t0 = Clock::now();
     std::unordered_map<std::string, int> refOrdinal;                  // path -> first position in the reference list
     for (size_t j = 0; j < parameters.refSequences.size(); j++) refOrdinal.emplace(parameters.refSequences[j], (int)j);
-    const bool deriveQueries = loading && G == 1 && !parameters.visualize;
+    const char *hostCgiEnv = getenv("BANI_CLI_HOST_CGI");
+    const bool hostCgi = parameters.visualize && hostCgiEnv && atoi(hostCgiEnv) != 0;     // per-query host computeCGI (test switch)
+    const bool deriveQueries = loading && G == 1 && !hostCgi;
     auto derivable = [&](const std::string &q) { return deriveQueries && refOrdinal.count(q) > 0; };
     std::unordered_map<std::string, int> pathId; std::vector<std::string> paths;
     for (const auto &e : parameters.querySequences) if (!derivable(e) && !pathId.count(e)) { pathId[e] = (int)paths.size(); paths.push_back(e); }
@@ -408,7 +412,7 @@ int main(int argc, char **argv)
           sanity[g] = referSketch.sanityCheck(parameters.maxRatioDiff); ratioDiffs[g] = referSketch.getRatioDifference();
           if (sanity[g]) {
             t1 = Clock::now();
-            if (parameters.visualize) {
+            if (hostCgi) {
               std::ostringstream vis;
               for (size_t q = 0; q < qrySlot.size(); q++) {
                 MappingResultsVector_t mapResults; uint64_t totalQueryFragments = 0;
@@ -429,12 +433,43 @@ int main(int argc, char **argv)
               if (!qh.empty()) { bani_qsketch *s = nullptr; check(bani_qsketch_create(ctx, qh.data(), (int32_t)qh.size(), qid.data(), referSketch.handle(), &s), "bani_qsketch_create"); sk.push_back(s); }
               if (!dord.empty()) { bani_qsketch *s = nullptr; check(bani_qsketch_from_index(ctx, referSketch.handle(), dord.data(), (int32_t)dord.size(), did.data(), &s), "bani_qsketch_from_index"); sk.push_back(s); }
               bani_cgi_result *res = nullptr; uint64_t n = 0; bani_map_counters ctr;
-              const int rc = bani_map_cgi_sketch(ctx, referSketch.handle(), sk.data(), (int32_t)sk.size(), &res, &n, &ctr);     // HP2 + reduction
+              bani_frag_mapping *frags = nullptr; uint64_t nf = 0;
+              const int rc = parameters.visualize                                                                  // HP2 + reduction
+                ? bani_map_cgi_sketch_frags(ctx, referSketch.handle(), sk.data(), (int32_t)sk.size(), &res, &n, &frags, &nf, &ctr)
+                : bani_map_cgi_sketch(ctx, referSketch.handle(), sk.data(), (int32_t)sk.size(), &res, &n, &ctr);
               for (auto *s : sk) bani_qsketch_destroy(s);
-              check(rc, "bani_map_cgi_sketch");
+              check(rc, parameters.visualize ? "bani_map_cgi_sketch_frags" : "bani_map_cgi_sketch");
               for (uint64_t i = 0; i < n; i++)
                 local.push_back(cgi::CGI_Results{res[i].refGenomeId, res[i].qryGenomeId, res[i].countSeq, res[i].totalQueryFragments, res[i].identity});
               bani_free(res);
+              if (parameters.visualize) {
+                // frags come per sketch (queries read, then queries derived): .visual lines go in query-list order.  The
+                // frags of one query are contiguous and in bin order, so a stable sort by query keeps that order.
+                std::stable_sort(frags, frags + nf, [](const bani_frag_mapping &a, const bani_frag_mapping &b) { return a.qryGenomeId < b.qryGenomeId; });
+                std::vector<skch::offset_t> refLens;
+                for (const auto &c : referSketch.metadata) refLens.push_back(c.len);
+                const std::vector<int64_t> refOff = cgi::offsetAdder(refLens);
+                std::ostringstream vis;
+                for (uint64_t i = 0; i < nf;) {
+                  const int32_t q = frags[i].qryGenomeId;
+                  uint64_t j = i;
+                  while (j < nf && frags[j].qryGenomeId == q) j++;
+                  // Map::metadata of the query: from its file, or (derived query) from its contigs in the index
+                  std::vector<skch::offset_t> qLens;
+                  if (qrySlot[q] >= 0) {
+                    for (const auto &c : dev[qrySlot[q]]->host->contigs) appendFragmentLengths(parameters, (offset_t)c.len, qLens);
+                  } else {
+                    const int o = refOrdinal.at(parameters.querySequences[q]);
+                    const int c0 = o ? referSketch.sequencesByFileInfo[o - 1] : 0, c1 = referSketch.sequencesByFileInfo[o];
+                    for (int c = c0; c < c1; c++) appendFragmentLengths(parameters, referSketch.metadata[c].len, qLens);
+                  }
+                  cgi::outputVisualizationFile(parameters, frags + i, j - i, cgi::offsetAdder(qLens), refOff, referSketch,
+                                               parameters.querySequences[q], shardRefNames, vis);
+                  i = j;
+                }
+                visual[g] = vis.str();
+              }
+              bani_free(frags);
             }
             if (g == 0) std::cerr << "INFO [GPU 0], skch::main, Time spent mapping " << qrySlot.size() << " query genome(s) : "
                                   << std::chrono::duration<double>(Clock::now() - t1).count() << " sec" << std::endl;

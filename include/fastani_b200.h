@@ -74,6 +74,15 @@ typedef struct {
   float   identity;
 } bani_cgi_result;
 
+/* One 2-way mapping behind a bani_cgi_result (cgi::MappingResult_CGI, cgid_types.hpp:18-28; 20 bytes): the fragment
+ * querySeqId (the reference's seqCounter: fragments of a query genome in order, a contig shorter than a fragment
+ * counting as one id) of query qryGenomeId won the position bin refStartPos / (fragLen - 20) of contig refSeqId (the
+ * contig ordinal inside the index) with this identity.  What outputVisualizationFile writes one .visual line for. */
+typedef struct {
+  int32_t qryGenomeId, querySeqId, refSeqId, refStartPos;
+  float   identity;
+} bani_frag_mapping;
+
 /* Integer work counters of one mapping call; SURVEY.md section 8(d) defines the
  * algorithmic bytes of HP2 from these (same meaning as the oracle's counters). */
 typedef struct {
@@ -329,6 +338,17 @@ BANI_API int  bani_qsketch_merge(bani_ctx *ctx, const bani_qsketch *const *sketc
 /* bani_map_cgi for prebuilt sketches (all on this context's device); results ordered by (sketch, query, refGenomeId). */
 BANI_API int  bani_map_cgi_sketch(bani_ctx *ctx, const bani_index *ix, const bani_qsketch *const *sketches, int32_t n_sketches,
                                   bani_cgi_result **results, uint64_t *n_results, bani_map_counters *counters);
+/* bani_map_cgi_sketch that also returns the 2-way mappings behind every result (what --visualize writes).
+ * - results are byte for byte those of bani_map_cgi_sketch.
+ * - frags are ordered by (sketch, query, refSeqId, refStartPos / (fragLen - 20)).
+ * - The frags of one (query, reference genome) pair number countSeq; their float32 sum in that order, divided by
+ *   countSeq, is identity.
+ * - Among fragments of equal identity in one bin, the largest querySeqId wins (computeCGI's stable sort).
+ * Both arrays are allocated by the library (free with bani_free).  The reduction's bin table holds 8 bytes per bin
+ * instead of 4, so a pass covers half as many queries. */
+BANI_API int  bani_map_cgi_sketch_frags(bani_ctx *ctx, const bani_index *ix, const bani_qsketch *const *sketches, int32_t n_sketches,
+                                        bani_cgi_result **results, uint64_t *n_results, bani_frag_mapping **frags, uint64_t *n_frags,
+                                        bani_map_counters *counters);
 
 BANI_API void bani_free(void *p);
 
