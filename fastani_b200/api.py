@@ -125,6 +125,9 @@ def load_library():
         "bani_plan_chunks": (C.c_int, [vp, vp, i32, i32, i32, u64, vp, P(i32)]),
         "bani_qsketch_bytes_estimate": (C.c_int, [u64, i32, i32, P(u64)]),
         "bani_parse_byte_count": (C.c_int, [C.c_char_p, P(u64)]),
+        "bani_index_file_info": (C.c_int, [C.c_char_p, P(i32), P(i32), P(i32), P(i32), P(i32), P(u64), P(u64), vp, vp, vp, vp, u64, vp, u64]),
+        "bani_index_load_budget": (C.c_int, [vp, C.c_char_p, i32, u64, P(vp), P(i32), P(u64)]),
+        "bani_qsketch_from_index_file": (C.c_int, [vp, C.c_char_p, vp, i32, vp, P(vp)]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)          # AttributeError if the ABI lost a symbol
@@ -144,7 +147,8 @@ EXPORTED_SYMBOLS = [
     "bani_map_cgi", "bani_free", "bani_synth_genome", "bani_qsketch_create", "bani_qsketch_destroy", "bani_qsketch_info",
     "bani_qsketch_export", "bani_qsketch_import", "bani_qsketch_merge", "bani_map_cgi_sketch", "bani_map_cgi_sketch_frags",
     "bani_index_build_budget", "bani_ctx_mem_stats", "bani_ctx_trim", "bani_ctx_plan_run", "bani_plan_run", "bani_run_working_set", "bani_index_footprint",
-    "bani_map_working_set", "bani_index_budget", "bani_plan_chunks", "bani_qsketch_bytes_estimate", "bani_parse_byte_count"]
+    "bani_map_working_set", "bani_index_budget", "bani_plan_chunks", "bani_qsketch_bytes_estimate", "bani_parse_byte_count",
+    "bani_index_file_info", "bani_index_load_budget", "bani_qsketch_from_index_file"]
 
 
 def _check(rc):
@@ -463,6 +467,20 @@ class Sketch:
         contig names from `names` (optional list, one per contig)."""
         h = C.c_void_p()
         _check(ctx.lib.bani_index_load(ctx.h, os.fsencode(path), C.byref(h)))
+        return cls._loaded(ctx, h, names)
+
+    @classmethod
+    def load_budget(cls, ctx, path, first, max_bytes, names=None):
+        """bani_index_load_budget: the index of the longest run of genomes of a saved file, from genome `first`, whose load
+        fits max_bytes (at least one genome); only that run is read.  names: optional, one per contig of the run.
+        Returns (Sketch, n_taken, peak_bytes)."""
+        h = C.c_void_p(); n = C.c_int32(); peak = C.c_uint64()
+        _check(ctx.lib.bani_index_load_budget(ctx.h, os.fsencode(path), int(first), int(max_bytes), C.byref(h), C.byref(n),
+                                              C.byref(peak)))
+        return cls._loaded(ctx, h, names), n.value, peak.value
+
+    @classmethod
+    def _loaded(cls, ctx, h, names):
         sk = cls(ctx, None, _handle=h)
         st = sk.stats()
         cl = np.zeros(max(st["n_contigs"], 1), np.int32); sbf = np.zeros(max(st["n_genomes"], 1), np.int32)
@@ -580,6 +598,16 @@ class QuerySketch:
         assert len(ids) == len(ords)
         h = C.c_void_p()
         _check(ctx.lib.bani_qsketch_from_index(ctx.h, sketch.h, ords.ctypes.data, len(ords), ids.ctypes.data, C.byref(h)))
+        return cls(ctx, _handle=h)
+
+    @classmethod
+    def from_index_file(cls, ctx, path, genome_ordinals, query_ids=None):
+        """from_index for genomes of a saved index file, reading only their records (bani_qsketch_from_index_file)."""
+        ords = np.ascontiguousarray(genome_ordinals, dtype=np.int32)
+        ids = np.ascontiguousarray(query_ids if query_ids is not None else genome_ordinals, dtype=np.int32)
+        assert len(ids) == len(ords)
+        h = C.c_void_p()
+        _check(ctx.lib.bani_qsketch_from_index_file(ctx.h, os.fsencode(path), ords.ctypes.data, len(ords), ids.ctypes.data, C.byref(h)))
         return cls(ctx, _handle=h)
 
     @classmethod
@@ -760,6 +788,68 @@ def compute_cgi_chunked(ctx, ref_contig_lists, query_sketches, index_budget=None
             for g in pending[:taken]:
                 g.close()
             pending = pending[taken:]
+            res, _ = compute_cgi_sketched(ctx, sk, qs[q0:q1])
+            res["refGenomeId"] += first
+            parts.append(res)
+            sk.close()
+            ctx.trim()
+            if bi == 0:
+                plan["chunks"].append((first, first + taken))
+                m = ctx.mem_stats()
+                plan["device_bytes"].append(m["live"] + m["cached"])
+            first += taken
+    out = np.concatenate(parts) if parts else np.empty(0, CGI_DTYPE)
+    out = out[np.lexsort((out["refGenomeId"], out["qryGenomeId"]))]
+    return out, plan
+
+
+def index_file_info(path):
+    """Header and tables of a saved index file (bani_index_file_info; no GPU needed): {"version", "k", "w", "frag_len",
+    "n_genomes", "n_contigs", "n_minimizers"} and per genome numpy arrays "genome_contigs", "genome_length" (bases),
+    "genome_records" (minimizers), "genome_bits" (validity bitmap bits), and "contig_length" in seqId order."""
+    lib = load_library()
+    p = os.fsencode(path)
+    ver, k, w, fl, ng = (C.c_int32() for _ in range(5))
+    nc, nm = C.c_uint64(), C.c_uint64()
+    scalars = [C.byref(x) for x in (ver, k, w, fl, ng, nc, nm)]
+    _check(lib.bani_index_file_info(p, *scalars, None, None, None, None, 0, None, 0))
+    gc = np.zeros(max(ng.value, 1), np.int32); gl = np.zeros(max(ng.value, 1), np.uint64)
+    gr = np.zeros(max(ng.value, 1), np.uint64); gb = np.zeros(max(ng.value, 1), np.uint64)
+    cl = np.zeros(max(nc.value, 1), np.int32)
+    _check(lib.bani_index_file_info(p, *scalars, gc.ctypes.data, gl.ctypes.data, gr.ctypes.data, gb.ctypes.data, len(gc),
+                                    cl.ctypes.data, len(cl)))
+    n, m = ng.value, nc.value
+    return {"version": ver.value, "k": k.value, "w": w.value, "frag_len": fl.value, "n_genomes": n, "n_contigs": m,
+            "n_minimizers": nm.value, "genome_contigs": gc[:n], "genome_length": gl[:n], "genome_records": gr[:n],
+            "genome_bits": gb[:n], "contig_length": cl[:m]}
+
+
+def compute_cgi_from_index_file(ctx, path, query_sketches, index_budget=None, query_budget=None):
+    """compute_cgi_chunked against the genomes of a saved index file (Sketch.save), which need not fit the device at once:
+    Context.plan_run plans chunks and query blocks from the file's genome lengths (index_file_info); if the run needs more
+    than one chunk or block, every block is mapped against the file's genomes loaded in runs that fit the index budget
+    (Sketch.load_budget from genome 0 until every genome is taken).  refGenomeId is the genome's ordinal in the file.  A
+    run of one chunk and one block is Sketch.load + compute_cgi_sketched.
+    Returns (results[CGI_DTYPE] ordered by (query, ref), plan) with the keys of compute_cgi_chunked; "chunks" are the runs
+    that were loaded."""
+    info = index_file_info(path)
+    n = info["n_genomes"]
+    qs = list(query_sketches)
+    infos = [q.info() for q in qs]
+    qlen = [x["n_hashes"] * (ctx.windowSize + 1) // 2 for x in infos]
+    planned, blocks, ib = ctx.plan_run(info["genome_length"], info["genome_contigs"], qlen, [x["export_bytes"] for x in infos],
+                                       index_budget or 0, query_budget or 0)
+    plan = {"chunks": [], "blocks": blocks, "index_budget": ib, "device_bytes": []}
+    if len(planned) <= 1 and len(blocks) <= 1:                    # fits: one index, one mapping call
+        sk = Sketch.load(ctx, path)
+        res, _ = compute_cgi_sketched(ctx, sk, qs)
+        plan["chunks"] = [(0, n)]
+        return res, plan
+    parts = []
+    for bi, (q0, q1) in enumerate(blocks):
+        first = 0
+        while first < n:
+            sk, taken, _ = Sketch.load_budget(ctx, path, first, ib)
             res, _ = compute_cgi_sketched(ctx, sk, qs[q0:q1])
             res["refGenomeId"] += first
             parts.append(res)

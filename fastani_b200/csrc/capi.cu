@@ -585,6 +585,52 @@ int bani_index_load(bani_ctx *ctx, const char *path, bani_index **out)
   BANI_CATCH
 }
 
+int bani_index_file_info(const char *path, int32_t *version, int32_t *k, int32_t *w, int32_t *frag_len, int32_t *n_genomes,
+                         uint64_t *n_contigs, uint64_t *n_minimizers, int32_t *genome_contigs, uint64_t *genome_len, uint64_t *genome_records,
+                         uint64_t *genome_bits, uint64_t cap_genomes, int32_t *contig_len, uint64_t cap_contigs)
+{
+  BANI_TRY
+  if (!path) fail(BANI_ERR_ARG, "null path");
+  const IndexFileInfo x = index_file_info(path);
+  const uint64_t nG = x.nGenomes, nC = x.nContigs;
+  if ((genome_contigs || genome_len || genome_records || genome_bits) && cap_genomes < nG) fail(BANI_ERR_ARG, "genome buffer too small");
+  if (contig_len && cap_contigs < nC) fail(BANI_ERR_ARG, "contig buffer too small");
+  for (uint64_t g = 0; g < nG; g++) {
+    const uint64_t c0 = x.contig_begin((int32_t)g), c1 = (uint64_t)x.seqsByFile[g];
+    uint64_t len = 0;
+    for (uint64_t c = c0; c < c1; c++) len += (uint64_t)x.contigLen[c];
+    if (genome_contigs) genome_contigs[g] = (int32_t)(c1 - c0);
+    if (genome_len) genome_len[g] = len;
+    if (genome_records) genome_records[g] = x.recOff[c1] - x.recOff[c0];
+    if (genome_bits) genome_bits[g] = x.bitOff[c1] - x.bitOff[c0];
+  }
+  if (contig_len && nC) memcpy(contig_len, x.contigLen.data(), 4 * nC);
+  if (version) *version = x.version;
+  if (k) *k = x.k;
+  if (w) *w = x.w;
+  if (frag_len) *frag_len = x.fragLen;
+  if (n_genomes) *n_genomes = (int32_t)nG;
+  if (n_contigs) *n_contigs = nC;
+  if (n_minimizers) *n_minimizers = x.M;
+  return BANI_OK;
+  BANI_CATCH
+}
+
+int bani_index_load_budget(bani_ctx *ctx, const char *path, int32_t first_genome, uint64_t max_bytes, bani_index **out, int32_t *n_taken,
+                           uint64_t *peak_bytes)
+{
+  BANI_TRY
+  if (!ctx || !path || !out || !n_taken) fail(BANI_ERR_ARG, "null argument");
+  BANI_CUDA(cudaSetDevice(ctx->c.device));
+  int32_t taken = 0; uint64_t peak = 0;
+  Index *ix = index_load_budget(&ctx->c, path, first_genome, max_bytes, &taken, &peak);
+  bani_index *h = new bani_index(); h->ix = ix; *out = h;
+  *n_taken = taken;
+  if (peak_bytes) *peak_bytes = peak;
+  return BANI_OK;
+  BANI_CATCH
+}
+
 int bani_index_contigs(const bani_index *ix, int32_t *contig_len, uint64_t cap_contigs, int32_t *seqs_by_file, uint64_t cap_genomes)
 {
   BANI_TRY
@@ -720,6 +766,19 @@ int bani_qsketch_from_index(bani_ctx *ctx, const bani_index *ix, const int32_t *
   BANI_CUDA(cudaSetDevice(ctx->c.device));
   std::unique_ptr<bani_qsketch> h(new bani_qsketch());
   h->qs = qsketch_from_index(&ctx->c, ix->ix, genome_ordinals, n_queries, query_ids);
+  *out = h.release();
+  return BANI_OK;
+  BANI_CATCH
+}
+
+int bani_qsketch_from_index_file(bani_ctx *ctx, const char *path, const int32_t *genome_ordinals, int32_t n_queries,
+                                 const int32_t *query_ids, bani_qsketch **out)
+{
+  BANI_TRY
+  if (!ctx || !path || n_queries < 0 || (n_queries && !genome_ordinals) || !out) fail(BANI_ERR_ARG, "null argument");
+  BANI_CUDA(cudaSetDevice(ctx->c.device));
+  std::unique_ptr<bani_qsketch> h(new bani_qsketch());
+  h->qs = qsketch_from_index_file(&ctx->c, path, genome_ordinals, n_queries, query_ids);
   *out = h.release();
   return BANI_OK;
   BANI_CATCH

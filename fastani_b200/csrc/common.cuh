@@ -364,6 +364,30 @@ int32_t plan_run(const RunSize &r, const uint64_t *refLen, const int32_t *refCon
 bool     parse_byte_count(const char *s, uint64_t *out);
 void   index_save(Ctx *ctx, const Index *ix, const char *path);
 Index *index_load(Ctx *ctx, const char *path);
+// Header and tables of a saved index (host only, index.cu: file layout), checked as index_load checks them and, from
+// version 3 on, against the table checksum.  Genome g owns contigs [contig_begin(g), seqsByFile[g]), records
+// [recOff[c0], recOff[c1]) and validity bits [bitOff[c0], bitOff[c1]).
+struct IndexFileInfo {
+  int version = 0, k = 0, w = 0, fragLen = 0;
+  uint64_t M = 0, nContigs = 0, nGenomes = 0, validWords = 0;
+  std::vector<int32_t> contigLen, seqsByFile;
+  std::vector<uint32_t> recOff;                 // nContigs + 1
+  std::vector<uint64_t> bitOff;                 // nContigs + 1: first validity bit of every contig (multiples of 32)
+  uint64_t contig_begin(int32_t g) const { return g ? (uint64_t)seqsByFile[g - 1] : 0; }
+  uint64_t off_hash() const;                    // byte offsets of the file's sections
+  uint64_t off_wpos() const { return off_hash() + 4 * M; }
+  uint64_t off_bits() const { return off_wpos() + 4 * M; }
+  uint64_t off_sums() const;
+  uint64_t file_bytes() const;
+};
+IndexFileInfo index_file_info(const char *path);
+// The longest run of genomes [first, first + *nTaken) of a version-3 file whose load (index_footprint of its exact record
+// count, no sketch staging) fits maxBytes, at least one (BANI_ERR_LIMIT if that one does not fit); only that run is read.
+// The index equals index_build's of exactly those genomes.  *peakBytes: most bytes held above the entry.
+Index *index_load_budget(Ctx *ctx, const char *path, int32_t first, uint64_t maxBytes, int32_t *nTaken, uint64_t *peakBytes);
+struct QSketch;
+// qsketch_from_index over the genomes `ordinals` of a version-3 file, reading only their records
+QSketch *qsketch_from_index_file(Ctx *ctx, const char *path, const int32_t *ordinals, int32_t nq, const int32_t *queryIds);
 
 // map.cu
 struct MapOutput {
@@ -377,6 +401,9 @@ void map_queries(Ctx *ctx, const Index *ix, const Genome *const *queries, int32_
                  bool wantRows, bool wantCgi, MapOutput &out);
 QSketch *qsketch_create(Ctx *ctx, const Genome *const *queries, int32_t nq, const int32_t *queryIds, const Index *hint);
 QSketch *qsketch_from_index(Ctx *ctx, const Index *ix, const int32_t *ordinals, int32_t nq, const int32_t *queryIds);
+// the same without the check that the index holds records: stage A' reads only contigRecOff, wpos, hash, the validity
+// bitmap and the contig tables, so `ix` may be a partial index read from a file (index.cu) without index_finish
+QSketch *qsketch_from_records(Ctx *ctx, const Index *ix, const int32_t *ordinals, int32_t nq, const int32_t *queryIds);
 uint64_t qsketch_export_bytes(const QSketch *qs);
 void qsketch_export(Ctx *ctx, const QSketch *qs, void *devBuf, uint64_t cap);
 QSketch *qsketch_import(Ctx *ctx, const void *devBuf, uint64_t bytes);

@@ -486,21 +486,29 @@ Index *index_build(Ctx *ctx, Genome *const *refs, int32_t nRefs)
   return index_build_impl(ctx, refs, nRefs, 0, &n);
 }
 
-Index *index_build_budget(Ctx *ctx, Genome *const *refs, int32_t nRefs, uint64_t maxBytes, int32_t *nTaken, uint64_t *peakBytes)
+// make(): *peakBytes = the most device memory held during the call above what was held on entry
+template <typename F>
+static Index *with_peak(Ctx *ctx, uint64_t *peakBytes, F &&make)
 {
-  if (nRefs < 1) fail(BANI_ERR_ARG, "a budgeted index build needs at least one genome");
-  if (maxBytes == 0) fail(BANI_ERR_ARG, "the index budget must be positive");
   size_t live0 = 0, peak0 = 0, peak = 0;
   dev_mem_stats(ctx->device, &live0, nullptr, &peak0);
   dev_mem_peak_set(ctx->device, 0);                        // high-water mark from here on
   Index *ix = nullptr;
-  try { ix = index_build_impl(ctx, refs, nRefs, maxBytes, nTaken); }
+  try { ix = make(); }
   catch (...) { dev_mem_stats(ctx->device, nullptr, nullptr, &peak); dev_mem_peak_set(ctx->device, std::max(peak0, peak)); throw; }
   dev_mem_stats(ctx->device, nullptr, nullptr, &peak);
   dev_mem_peak_set(ctx->device, std::max(peak0, peak));
   *peakBytes = peak > live0 ? peak - live0 : 0;
   return ix;
 }
+
+Index *index_build_budget(Ctx *ctx, Genome *const *refs, int32_t nRefs, uint64_t maxBytes, int32_t *nTaken, uint64_t *peakBytes)
+{
+  if (nRefs < 1) fail(BANI_ERR_ARG, "a budgeted index build needs at least one genome");
+  if (maxBytes == 0) fail(BANI_ERR_ARG, "the index budget must be positive");
+  return with_peak(ctx, peakBytes, [&] { return index_build_impl(ctx, refs, nRefs, maxBytes, nTaken); });
+}
+
 
 // ---------------------------------------------------------------------------------------- on-disk sketch cache (SURVEY 8 f-4)
 // The reference has no cache (only scripts/splitDatabase.sh + README.md:104-106: "divide the database, run as parallel
@@ -511,8 +519,16 @@ Index *index_build_budget(Ctx *ctx, Genome *const *refs, int32_t nRefs, uint64_t
 // genomes (qsketch_from_index): an all-vs-all run against a cache reads no FASTA at all.
 //   u64 x 16 : magic, version, k, w, fragLen, M, nContigs, nGenomes, validWords, 0...
 //   i32 contigLen[nContigs] | i32 seqsByFile[nGenomes] | u32 contigRecOff[nContigs+1] | u32 hash[M] | i32 wpos[M] |
-//   u32 validBits[validWords] | u64 checksum (sum of all preceding 32-bit words)
+//   u32 validBits[validWords] |
+//   version 3 only: u64 tableSum | u64 genomeSum[nGenomes] |
+//   u64 checksum (sum of all preceding 32-bit words)
+// A sum is the 64-bit sum of the 32-bit words it covers.  tableSum covers the header, contigLen, seqsByFile and
+// contigRecOff; genomeSum[g] covers genome g's records -- its slices of hash and of wpos -- and its validity bitmap words
+// (every contig's bits start on a word, so a genome's bits are whole words).  The last bitmap word lies past every contig
+// and is zero.  So a run of genomes can be read and checked without reading the rest of the file (index_load_budget,
+// qsketch_from_index_file).  Version 2 files have the whole-file checksum only and are loaded whole.
 static constexpr uint64_t IX_MAGIC = 0x32584449494e4142ull;
+static constexpr uint64_t IX_HEADER_BYTES = 128;
 
 __global__ void seqid_fill_kernel(const uint32_t *contigRecOff, int32_t nC, int32_t *seqId)
 {
@@ -522,15 +538,134 @@ __global__ void seqid_fill_kernel(const uint32_t *contigRecOff, int32_t nC, int3
   for (uint32_t i = a + threadIdx.x; i < b; i += blockDim.x) seqId[i] = c;
 }
 
+static uint64_t word_sum(const void *p, size_t bytes)
+{
+  const uint32_t *w = (const uint32_t *)p;
+  uint64_t s = 0;
+  for (size_t i = 0; i < bytes / 4; i++) s += w[i];
+  return s;
+}
+
 namespace {
 struct File {
   FILE *f = nullptr; std::string path; uint64_t sum = 0;
   File(const char *p, const char *mode) : f(fopen(p, mode)), path(p) { if (!f) fail(BANI_ERR_ARG, "cannot open %s", p); }
   ~File() { if (f) fclose(f); }
-  void write(const void *p, size_t n) { if (n && fwrite(p, 1, n, f) != n) fail(BANI_ERR_INTERNAL, "write error on %s", path.c_str()); add(p, n); }
-  void read(void *p, size_t n) { if (n && fread(p, 1, n, f) != n) fail(BANI_ERR_ARG, "%s is truncated", path.c_str()); add(p, n); }
-  void add(const void *p, size_t n) { const uint32_t *w = (const uint32_t *)p; uint64_t s = 0; for (size_t i = 0; i < n / 4; i++) s += w[i]; sum += s; }
+  void write(const void *p, size_t n) { if (n && fwrite(p, 1, n, f) != n) fail(BANI_ERR_INTERNAL, "write error on %s", path.c_str()); sum += word_sum(p, n); }
+  void read(void *p, size_t n) { if (n && fread(p, 1, n, f) != n) fail(BANI_ERR_ARG, "%s is truncated", path.c_str()); sum += word_sum(p, n); }
+  void seek(uint64_t off) { if (fseeko(f, (off_t)off, SEEK_SET) != 0) fail(BANI_ERR_ARG, "%s: cannot seek to byte %llu", path.c_str(), (unsigned long long)off); }
 };
+
+// Disk -> device through two pinned buffers: the disk read of a piece overlaps the copy of the previous one.
+struct Upload {
+  static constexpr size_t CH = (size_t)64 << 20;
+  cudaStream_t st; File &f;
+  void *stage[2] = {nullptr, nullptr};
+  cudaEvent_t ev[2] = {nullptr, nullptr};
+  int cur = 0; bool used[2] = {false, false};
+  Upload(Ctx *ctx, File &file) : st(ctx->stream), f(file)
+  {
+    try {
+      BANI_CUDA(cudaHostAlloc(&stage[0], CH, cudaHostAllocDefault));
+      BANI_CUDA(cudaHostAlloc(&stage[1], CH, cudaHostAllocDefault));
+      BANI_CUDA(cudaEventCreate(&ev[0])); BANI_CUDA(cudaEventCreate(&ev[1]));
+    } catch (...) { release(); throw; }
+  }
+  ~Upload() { release(); }
+  void release()
+  {
+    cudaStreamSynchronize(st);
+    for (int i = 0; i < 2; i++) {
+      if (stage[i]) cudaFreeHost(stage[i]);
+      if (ev[i]) cudaEventDestroy(ev[i]);
+      stage[i] = nullptr; ev[i] = nullptr;
+    }
+  }
+  // `bytes` from the file's current position to device address dp; *sum (optional) += their word sum
+  void copy(void *dp, uint64_t bytes, uint64_t *sum = nullptr)
+  {
+    for (uint64_t o = 0; o < bytes; o += CH) {
+      const size_t n = (size_t)std::min<uint64_t>(CH, bytes - o);
+      if (used[cur]) BANI_CUDA(cudaEventSynchronize(ev[cur]));
+      f.read(stage[cur], n);
+      if (sum) *sum += word_sum(stage[cur], n);
+      BANI_CUDA(cudaMemcpyAsync((uint8_t *)dp + o, stage[cur], n, cudaMemcpyHostToDevice, st));
+      BANI_CUDA(cudaEventRecord(ev[cur], st));
+      used[cur] = true; cur ^= 1;
+    }
+  }
+  void finish() { BANI_CUDA(cudaStreamSynchronize(st)); }
+};
+}
+
+uint64_t IndexFileInfo::off_hash() const { return IX_HEADER_BYTES + 4 * nContigs + 4 * nGenomes + 4 * (nContigs + 1); }
+uint64_t IndexFileInfo::off_sums() const { return off_bits() + 4 * validWords; }
+uint64_t IndexFileInfo::file_bytes() const { return off_sums() + (version >= 3 ? 8 + 8 * nGenomes : 0) + 8; }
+
+// Header and tables of a saved index, checked as a whole load checks them and, version 3, against tableSum first (a
+// corrupt table is reported as such).  The file is left after contigRecOff, with f.sum the sum of everything read so far.
+static IndexFileInfo index_file_tables(File &f)
+{
+  const char *path = f.path.c_str();
+  IndexFileInfo x;
+  uint64_t h[16];
+  f.read(h, sizeof h);
+  if (h[0] != IX_MAGIC || (h[1] != 2 && h[1] != 3)) fail(BANI_ERR_ARG, "%s is not a fastani_b200 index file (version 2 or 3)", path);
+  x.version = (int)h[1]; x.k = (int)h[2]; x.w = (int)h[3]; x.fragLen = (int)h[4];
+  const uint64_t M = h[5], nC = h[6], nG = h[7];
+  x.M = M; x.nContigs = nC; x.nGenomes = nG; x.validWords = h[8];
+  if (M > 0xfffffff0ull || nC > 0x7ffffff0ull || nG > nC + 1 || nG > 0x7ffffff0ull || x.validWords > (1ull << 40))
+    fail(BANI_ERR_ARG, "%s: corrupt header", path);
+  {   // the sizes in the header must match the file before anything is allocated
+    if (fseeko(f.f, 0, SEEK_END) != 0) fail(BANI_ERR_ARG, "%s: cannot seek", path);
+    const uint64_t fileBytes = (uint64_t)ftello(f.f);
+    f.seek(sizeof h);
+    if (fileBytes != x.file_bytes())
+      fail(BANI_ERR_ARG, "%s: %llu bytes, header says %llu (truncated or corrupt)", path, (unsigned long long)fileBytes, (unsigned long long)x.file_bytes());
+  }
+  x.contigLen.resize(nC); x.seqsByFile.resize(nG); x.recOff.resize(nC + 1);
+  f.read(x.contigLen.data(), 4 * nC);
+  f.read(x.seqsByFile.data(), 4 * nG);
+  f.read(x.recOff.data(), 4 * (nC + 1));
+  if (x.version >= 3) {
+    uint64_t tableSum = 0;
+    const uint64_t pos = (uint64_t)ftello(f.f);
+    f.seek(x.off_sums());
+    if (fread(&tableSum, 1, 8, f.f) != 8) fail(BANI_ERR_ARG, "%s is truncated", path);
+    f.seek(pos);
+    if (tableSum != f.sum) fail(BANI_ERR_ARG, "%s: table checksum mismatch (header or contig tables corrupt)", path);
+  }
+  int32_t prev = 0;
+  for (uint64_t g = 0; g < nG; g++) {
+    const int32_t e = x.seqsByFile[g];
+    if (e < prev || (uint64_t)e > nC) fail(BANI_ERR_ARG, "%s: corrupt genome table", path);
+    prev = e;
+  }
+  if ((uint64_t)prev != nC) fail(BANI_ERR_ARG, "%s: corrupt genome table (it ends at contig %d of %llu)", path, prev, (unsigned long long)nC);
+  x.bitOff.assign(nC + 1, 0);
+  for (uint64_t c = 0; c < nC; c++) {
+    if (x.contigLen[c] < 0) fail(BANI_ERR_ARG, "%s: corrupt contig table", path);
+    x.bitOff[c + 1] = x.bitOff[c] + (((uint64_t)x.contigLen[c] + 31) & ~31ull);
+  }
+  for (uint64_t c = 0; c < nC; c++) if (x.recOff[c] > x.recOff[c + 1]) fail(BANI_ERR_ARG, "%s: corrupt record offsets", path);
+  if (x.recOff[0] != 0 || x.recOff[nC] != M) fail(BANI_ERR_ARG, "%s: corrupt record offsets", path);
+  if (M ? x.validWords != x.bitOff[nC] / 32 + 1 : x.validWords != 0)
+    fail(BANI_ERR_ARG, "%s: validity bitmap size does not match the contig table", path);
+  return x;
+}
+
+IndexFileInfo index_file_info(const char *path)
+{
+  File f(path, "rb");
+  return index_file_tables(f);
+}
+
+static void check_file_params(const Ctx *ctx, const IndexFileInfo &x, const char *path)
+{
+  const int k = ctx->prm.kmer_size, w = ctx->prm.window_size, fragLen = ctx->prm.frag_len;
+  if (x.k != k || x.w != w || x.fragLen != fragLen)
+    fail(BANI_ERR_ARG, "%s was built with other parameters (k %d w %d fragLen %d), this context has k %d w %d fragLen %d",
+         path, x.k, x.w, x.fragLen, k, w, fragLen);
 }
 
 void index_save(Ctx *ctx, const Index *ix, const char *path)
@@ -540,121 +675,213 @@ void index_save(Ctx *ctx, const Index *ix, const char *path)
   File f(path, "wb");
   const uint64_t M = ix->M, nC = (uint64_t)ix->nContigs, nG = (uint64_t)ix->nGenomes;
   const uint64_t validWords = M ? ix->validBits.n : 0;
-  uint64_t h[16] = {IX_MAGIC, 2, (uint64_t)ix->k, (uint64_t)ix->w, (uint64_t)ix->fragLen, M, nC, nG, validWords};
+  uint64_t h[16] = {IX_MAGIC, 3, (uint64_t)ix->k, (uint64_t)ix->w, (uint64_t)ix->fragLen, M, nC, nG, validWords};
   f.write(h, sizeof h);
   f.write(ix->contigLen.data(), 4 * nC);
   f.write(ix->seqsByFile.data(), 4 * nG);
+  std::vector<uint32_t> recOff(nC + 1);
+  BANI_CUDA(cudaMemcpyAsync(recOff.data(), ix->contigRecOff.p, 4 * (nC + 1), cudaMemcpyDeviceToHost, st));
+  BANI_CUDA(cudaStreamSynchronize(st));
+  f.write(recOff.data(), 4 * (nC + 1));
+  const uint64_t tableSum = f.sum;
+  // where every genome's records and bitmap words end (in 32-bit words of the hash / wpos and validBits arrays)
+  std::vector<uint64_t> recEnd(nG), bitEnd(nG);
+  {
+    uint64_t bits = 0;
+    for (uint64_t g = 0, c = 0; g < nG; g++) {
+      for (; c < (uint64_t)ix->seqsByFile[g]; c++) bits += ((uint64_t)ix->contigLen[c] + 31) & ~31ull;
+      recEnd[g] = recOff[ix->seqsByFile[g]];
+      bitEnd[g] = bits / 32;
+    }
+  }
+  std::vector<uint64_t> genomeSum(nG, 0);
   // device arrays through a pinned staging buffer
-  const size_t CH = (size_t)64 << 20;
+  const size_t CHW = (size_t)16 << 20;             // words per piece
   void *stage = nullptr;
-  BANI_CUDA(cudaHostAlloc(&stage, CH, cudaHostAllocDefault));
+  BANI_CUDA(cudaHostAlloc(&stage, 4 * CHW, cudaHostAllocDefault));
   try {
-    auto dump = [&](const void *dp, uint64_t bytes) {
-      for (uint64_t o = 0; o < bytes; o += CH) {
-        const size_t n = (size_t)std::min<uint64_t>(CH, bytes - o);
-        BANI_CUDA(cudaMemcpyAsync(stage, (const uint8_t *)dp + o, n, cudaMemcpyDeviceToHost, st));
+    auto dump = [&](const void *dp, uint64_t words, const std::vector<uint64_t> &ends) {
+      size_t g = 0;
+      for (uint64_t o = 0; o < words; o += CHW) {
+        const uint64_t n = std::min<uint64_t>(CHW, words - o);
+        BANI_CUDA(cudaMemcpyAsync(stage, (const uint32_t *)dp + o, 4 * n, cudaMemcpyDeviceToHost, st));
         BANI_CUDA(cudaStreamSynchronize(st));
-        f.write(stage, n);
+        f.write(stage, 4 * n);
+        const uint32_t *w = (const uint32_t *)stage;
+        for (uint64_t i = 0; i < n;) {                  // words past the last genome (the trailing bitmap word) count for none
+          while (g < ends.size() && ends[g] <= o + i) g++;
+          if (g == ends.size()) break;
+          const uint64_t e = std::min<uint64_t>(n, ends[g] - o);
+          genomeSum[g] += word_sum(w + i, 4 * (e - i));
+          i = e;
+        }
       }
     };
-    dump(ix->contigRecOff.p, 4 * (nC + 1));
-    dump(ix->hash.p, 4 * M); dump(ix->wpos.p, 4 * M);
-    dump(ix->validBits.p, 4 * validWords);
+    dump(ix->hash.p, M, recEnd); dump(ix->wpos.p, M, recEnd);
+    dump(ix->validBits.p, validWords, bitEnd);
   } catch (...) { cudaFreeHost(stage); throw; }
   cudaFreeHost(stage);
+  f.write(&tableSum, 8);
+  f.write(genomeSum.data(), 8 * nG);
   const uint64_t sum = f.sum;
   f.write(&sum, 8);
+}
+
+// rebuilds the hash-ordered side of an index whose position-ordered side was read from a file
+static void index_finish_loaded(Ctx *ctx, Index *ix)
+{
+  if (ix->M == 0) { index_make_empty(ctx, ix); return; }
+  ix->seqId.alloc(ix->M, ctx->stream);
+  seqid_fill_kernel<<<(unsigned)ix->nContigs, 128, 0, ctx->stream>>>(ix->contigRecOff.p, ix->nContigs, ix->seqId.p);
+  ctx->launches++;
+  index_finish(ctx, ix);
 }
 
 Index *index_load(Ctx *ctx, const char *path)
 {
   cudaStream_t st = ctx->stream;
   File f(path, "rb");
-  uint64_t h[16];
-  f.read(h, sizeof h);
-  if (h[0] != IX_MAGIC || h[1] != 2) fail(BANI_ERR_ARG, "%s is not a fastani_b200 index file (version 2)", path);
-  const int k = ctx->prm.kmer_size, w = ctx->prm.window_size, fragLen = ctx->prm.frag_len;
-  if ((int)h[2] != k || (int)h[3] != w || (int)h[4] != fragLen)
-    fail(BANI_ERR_ARG, "%s was built with other parameters (k %d w %d fragLen %d), this context has k %d w %d fragLen %d",
-         path, (int)h[2], (int)h[3], (int)h[4], k, w, fragLen);
-  const uint64_t M = h[5], nC = h[6], nG = h[7], validWords = h[8];
-  if (M > 0xfffffff0ull || nC > 0x7ffffff0ull || nG > nC + 1 || nG > 0x7ffffff0ull) fail(BANI_ERR_ARG, "%s: corrupt header", path);
-  {   // the sizes in the header must match the file before anything is allocated
-    const long pos = ftell(f.f);
-    fseek(f.f, 0, SEEK_END);
-    const uint64_t fileBytes = (uint64_t)ftell(f.f);
-    fseek(f.f, pos, SEEK_SET);
-    const uint64_t want = sizeof h + 4 * nC + 4 * nG + 4 * (nC + 1) + 8 * M + 4 * validWords + 8;
-    if (fileBytes != want) fail(BANI_ERR_ARG, "%s: %llu bytes, header says %llu (truncated or corrupt)", path, (unsigned long long)fileBytes, (unsigned long long)want);
-  }
+  const IndexFileInfo x = index_file_tables(f);
+  check_file_params(ctx, x, path);
+  const uint64_t M = x.M, nC = x.contigLen.size(), nG = x.seqsByFile.size();
   auto ix = std::make_unique<Index>();
-  ix->device = ctx->device; ix->k = k; ix->w = w; ix->fragLen = fragLen; ix->nGenomes = (int32_t)nG;
-  ix->contigLen.resize(nC); ix->seqsByFile.resize(nG);
-  f.read(ix->contigLen.data(), 4 * nC);
-  f.read(ix->seqsByFile.data(), 4 * nG);
+  ix->device = ctx->device; ix->k = x.k; ix->w = x.w; ix->fragLen = x.fragLen; ix->nGenomes = (int32_t)nG;
+  ix->contigLen = x.contigLen; ix->seqsByFile = x.seqsByFile;
   std::vector<int32_t> contigGenome(nC);
+  for (uint64_t g = 0, c = 0; g < nG; g++) for (; c < (uint64_t)x.seqsByFile[g]; c++) contigGenome[c] = (int32_t)g;
+  index_contig_tables(ctx, ix.get(), contigGenome);
+  BANI_CUDA(cudaMemcpyAsync(ix->contigRecOff.p, x.recOff.data(), 4 * (nC + 1), cudaMemcpyHostToDevice, st));
+  ix->M = M;
   {
-    int32_t prev = 0;
-    for (uint64_t g = 0; g < nG; g++) {
-      const int32_t e = ix->seqsByFile[g];
-      if (e < prev || (uint64_t)e > nC) fail(BANI_ERR_ARG, "%s: corrupt genome table", path);
-      for (int32_t c = prev; c < e; c++) contigGenome[c] = (int32_t)g;
-      prev = e;
+    Upload up(ctx, f);
+    if (M) {
+      ix->hash.alloc(M, st); ix->wpos.alloc(M, st);
+      ix->validBits.alloc(x.validWords, st);
+      up.copy(ix->hash.p, 4 * M); up.copy(ix->wpos.p, 4 * M); up.copy(ix->validBits.p, 4 * x.validWords);
     }
-    if ((uint64_t)prev != nC) fail(BANI_ERR_ARG, "%s: corrupt genome table", path);
-    for (uint64_t c = 0; c < nC; c++) if (ix->contigLen[c] < 0) fail(BANI_ERR_ARG, "%s: corrupt contig table", path);
+    up.finish();
   }
-  const unsigned long long totalBits = index_contig_tables(ctx, ix.get(), contigGenome);
-  if (M && validWords != totalBits / 32 + 1) fail(BANI_ERR_ARG, "%s: validity bitmap size does not match the contig table", path);
-  const size_t CH = (size_t)64 << 20;
-  void *stage[2] = {nullptr, nullptr};
-  cudaEvent_t ev[2] = {nullptr, nullptr};
-  BANI_CUDA(cudaHostAlloc(&stage[0], CH, cudaHostAllocDefault));
-  BANI_CUDA(cudaHostAlloc(&stage[1], CH, cudaHostAllocDefault));
-  cudaEventCreate(&ev[0]); cudaEventCreate(&ev[1]);
-  auto cleanup = [&] { cudaStreamSynchronize(st); cudaFreeHost(stage[0]); cudaFreeHost(stage[1]); cudaEventDestroy(ev[0]); cudaEventDestroy(ev[1]); };
-  try {
-    int cur = 0; bool used[2] = {false, false};
-    auto slurp = [&](void *dp, uint64_t bytes) {          // disk read of chunk i+1 overlaps the H2D copy of chunk i
-      for (uint64_t o = 0; o < bytes; o += CH) {
-        const size_t n = (size_t)std::min<uint64_t>(CH, bytes - o);
-        if (used[cur]) BANI_CUDA(cudaEventSynchronize(ev[cur]));
-        f.read(stage[cur], n);
-        BANI_CUDA(cudaMemcpyAsync((uint8_t *)dp + o, stage[cur], n, cudaMemcpyHostToDevice, st));
-        BANI_CUDA(cudaEventRecord(ev[cur], st));
-        used[cur] = true; cur ^= 1;
-      }
-    };
-    slurp(ix->contigRecOff.p, 4 * (nC + 1));
-    if (M == 0) {
-      cudaStreamSynchronize(st);
-      uint64_t sum = f.sum, got = 0;
-      if (fread(&got, 1, 8, f.f) != 8 || got != sum) fail(BANI_ERR_ARG, "%s: checksum mismatch", path);
-      cleanup();
-      index_make_empty(ctx, ix.get());
-      return ix.release();
-    }
-    ix->M = M;
-    ix->hash.alloc(M, st); ix->wpos.alloc(M, st); ix->seqId.alloc(M, st);
-    ix->validBits.alloc(validWords, st);
-    slurp(ix->hash.p, 4 * M); slurp(ix->wpos.p, 4 * M); slurp(ix->validBits.p, 4 * validWords);
-    BANI_CUDA(cudaStreamSynchronize(st));
-    uint64_t sum = f.sum, got = 0;
-    if (fread(&got, 1, 8, f.f) != 8 || got != sum) fail(BANI_ERR_ARG, "%s: checksum mismatch", path);
-  } catch (...) { cleanup(); throw; }
-  cleanup();
-  // the record table must be consistent before it is used as an index: offsets ascending and ending at M
-  {
-    std::vector<uint32_t> ro(nC + 1);
-    BANI_CUDA(cudaMemcpyAsync(ro.data(), ix->contigRecOff.p, 4 * (nC + 1), cudaMemcpyDeviceToHost, st));
-    BANI_CUDA(cudaStreamSynchronize(st));
-    for (uint64_t c = 0; c < nC; c++) if (ro[c] > ro[c + 1]) fail(BANI_ERR_ARG, "%s: corrupt record offsets", path);
-    if (ro[0] != 0 || ro[nC] != M) fail(BANI_ERR_ARG, "%s: corrupt record offsets", path);
-  }
-  seqid_fill_kernel<<<(unsigned)nC, 128, 0, st>>>(ix->contigRecOff.p, (int32_t)nC, ix->seqId.p);
-  ctx->launches++;
-  index_finish(ctx, ix.get());
+  if (x.version >= 3) { std::vector<uint64_t> sums(1 + nG); f.read(sums.data(), 8 * sums.size()); }
+  const uint64_t sum = f.sum;
+  uint64_t got = 0;
+  if (fread(&got, 1, 8, f.f) != 8 || got != sum) fail(BANI_ERR_ARG, "%s: checksum mismatch", path);
+  index_finish_loaded(ctx, ix.get());
   return ix.release();
+}
+
+// Genomes `gs` (ascending, distinct) of a version-3 file as the position-ordered side of one index, as index_build would
+// have made it from exactly those genomes: contig tables, contigRecOff rebased to the genomes' records, hash, wpos and the
+// validity bitmap.  Every slice read is checked against its genome's sum before the index is returned.
+static std::unique_ptr<Index> index_read_genomes(Ctx *ctx, File &f, const IndexFileInfo &x, const std::vector<int32_t> &gs)
+{
+  cudaStream_t st = ctx->stream;
+  const char *path = f.path.c_str();
+  const uint64_t nG = x.seqsByFile.size();
+  auto ix = std::make_unique<Index>();
+  ix->device = ctx->device; ix->k = x.k; ix->w = x.w; ix->fragLen = x.fragLen; ix->nGenomes = (int32_t)gs.size();
+  std::vector<int32_t> contigGenome;
+  std::vector<uint32_t> recOff(1, 0);
+  for (size_t i = 0; i < gs.size(); i++) {
+    const int32_t g = gs[i];
+    const uint64_t c0 = x.contig_begin(g), c1 = x.seqsByFile[g], base = recOff.back();
+    for (uint64_t c = c0; c < c1; c++) {
+      ix->contigLen.push_back(x.contigLen[c]);
+      contigGenome.push_back((int32_t)i);
+      recOff.push_back((uint32_t)(base + x.recOff[c + 1] - x.recOff[c0]));
+    }
+    ix->seqsByFile.push_back((int32_t)ix->contigLen.size());
+  }
+  const uint64_t M = recOff.back(), nC = ix->contigLen.size();
+  const unsigned long long totalBits = index_contig_tables(ctx, ix.get(), contigGenome);
+  BANI_CUDA(cudaMemcpyAsync(ix->contigRecOff.p, recOff.data(), 4 * (nC + 1), cudaMemcpyHostToDevice, st));
+  ix->M = M;
+  std::vector<uint64_t> want(nG);
+  f.seek(x.off_sums() + 8);
+  f.read(want.data(), 8 * nG);
+  if (M) {
+    ix->hash.alloc(M, st); ix->wpos.alloc(M, st);
+    ix->validBits.alloc((size_t)(totalBits / 32) + 1, st);
+    BANI_CUDA(cudaMemsetAsync(ix->validBits.p, 0, ix->validBits.bytes(), st));
+    std::vector<uint64_t> got(gs.size(), 0);
+    Upload up(ctx, f);
+    uint64_t r = 0, b = 0;
+    for (size_t i = 0; i < gs.size(); i++) {
+      const int32_t g = gs[i];
+      const uint64_t r0 = x.recOff[x.contig_begin(g)], n = x.recOff[x.seqsByFile[g]] - r0;
+      f.seek(x.off_hash() + 4 * r0); up.copy(ix->hash.p + r, 4 * n, &got[i]);
+      f.seek(x.off_wpos() + 4 * r0); up.copy(ix->wpos.p + r, 4 * n, &got[i]);
+      const uint64_t w0 = x.bitOff[x.contig_begin(g)] / 32, nw = x.bitOff[x.seqsByFile[g]] / 32 - w0;
+      f.seek(x.off_bits() + 4 * w0); up.copy(ix->validBits.p + b, 4 * nw, &got[i]);
+      r += n; b += nw;
+    }
+    up.finish();
+    for (size_t i = 0; i < gs.size(); i++)
+      if (got[i] != want[gs[i]]) fail(BANI_ERR_ARG, "%s: checksum mismatch in genome %d", path, gs[i]);
+    if (gs.back() == (int32_t)nG - 1) {            // the trailing bitmap word belongs to no genome: it must be zero
+      uint32_t last = 1;
+      f.seek(x.off_bits() + 4 * (x.validWords - 1));
+      f.read(&last, 4);
+      if (last != 0) fail(BANI_ERR_ARG, "%s: corrupt validity bitmap (the word past the last contig is not zero)", path);
+    }
+  }
+  return ix;
+}
+
+static void require_ranges(const IndexFileInfo &x, const char *path)
+{
+  if (x.version < 3)
+    fail(BANI_ERR_ARG, "%s was saved in version 2, which has no per-genome checksums: load it whole, or save it again to load "
+         "it in ranges", path);
+}
+
+Index *index_load_budget(Ctx *ctx, const char *path, int32_t first, uint64_t maxBytes, int32_t *nTaken, uint64_t *peakBytes)
+{
+  if (maxBytes == 0) fail(BANI_ERR_ARG, "the index budget must be positive");
+  File f(path, "rb");
+  const IndexFileInfo x = index_file_tables(f);
+  check_file_params(ctx, x, path);
+  require_ranges(x, path);
+  const int32_t nG = (int32_t)x.seqsByFile.size();
+  if (first < 0 || first >= nG) fail(BANI_ERR_ARG, "genome %d outside %s (%d genomes)", first, path, nG);
+  // the longest run [first, first + t) whose load fits: the footprint of an index build without sketch staging
+  int32_t t = 0;
+  const uint64_t c0 = x.contig_begin(first);
+  auto need = [&](int32_t e) {
+    const uint64_t c1 = x.seqsByFile[e - 1], m = x.recOff[c1] - x.recOff[c0];
+    return index_footprint(m, m, c1 - c0, x.bitOff[c1] - x.bitOff[c0], 0).peak;
+  };
+  while (first + t < nG && need(first + t + 1) <= maxBytes) t++;
+  if (t == 0)
+    fail(BANI_ERR_LIMIT, "genome %d of %s (%llu minimizers) does not fit the index budget of %llu bytes: its index needs %llu", first, path,
+         (unsigned long long)(x.recOff[x.seqsByFile[first]] - x.recOff[c0]), (unsigned long long)maxBytes, (unsigned long long)need(first + 1));
+  *nTaken = t;
+  std::vector<int32_t> gs(t);
+  for (int32_t i = 0; i < t; i++) gs[i] = first + i;
+  return with_peak(ctx, peakBytes, [&] {
+    std::unique_ptr<Index> ix = index_read_genomes(ctx, f, x, gs);
+    index_finish_loaded(ctx, ix.get());
+    return ix.release();
+  });
+}
+
+QSketch *qsketch_from_index_file(Ctx *ctx, const char *path, const int32_t *ordinals, int32_t nq, const int32_t *queryIds)
+{
+  File f(path, "rb");
+  const IndexFileInfo x = index_file_tables(f);
+  check_file_params(ctx, x, path);
+  require_ranges(x, path);
+  const int32_t nG = (int32_t)x.seqsByFile.size();
+  for (int32_t i = 0; i < nq; i++)
+    if (ordinals[i] < 0 || ordinals[i] >= nG) fail(BANI_ERR_ARG, "genome ordinal %d outside %s (%d genomes)", ordinals[i], path, nG);
+  if (x.M == 0) fail(BANI_ERR_ARG, "%s holds no minimizers: query sketches cannot be derived from it", path);
+  // only the genomes asked for are read, each once, in file order; the queries keep their order
+  std::vector<int32_t> gs(ordinals, ordinals + nq);
+  std::sort(gs.begin(), gs.end());
+  gs.erase(std::unique(gs.begin(), gs.end()), gs.end());
+  std::vector<int32_t> local(nq);
+  for (int32_t i = 0; i < nq; i++) local[i] = (int32_t)(std::lower_bound(gs.begin(), gs.end(), ordinals[i]) - gs.begin());
+  std::unique_ptr<Index> part = index_read_genomes(ctx, f, x, gs);
+  return qsketch_from_records(ctx, part.get(), local.data(), nq, queryIds);
 }
 
 } // namespace bani

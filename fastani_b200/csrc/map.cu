@@ -1095,12 +1095,19 @@ QSketch *qsketch_create(Ctx *ctx, const Genome *const *queries, int32_t nq, cons
 }
 
 // Fragment sketches of genomes of the index itself, by genome ordinal: needs nothing but the index (an index loaded
-// from disk serves as the query side of an all-vs-all run without any FASTA being read).
+// from disk serves as the query side of an all-vs-all run without any FASTA being read).  qsketch_from_index_file
+// (index.cu) calls qsketch_from_records with a partial index of only the genomes asked for.
 QSketch *qsketch_from_index(Ctx *ctx, const Index *ix, const int32_t *ordinals, int32_t nq, const int32_t *queryIds)
 {
   if (ix->device != ctx->device) fail(BANI_ERR_ARG, "index lives on another device");
   if (ix->k != ctx->prm.kmer_size || ix->w != ctx->prm.window_size || ix->fragLen != ctx->prm.frag_len)
     fail(BANI_ERR_ARG, "index was built with other parameters (k %d w %d fragLen %d)", ix->k, ix->w, ix->fragLen);
+  if (ix->M == 0 || !ix->validBits.p) fail(BANI_ERR_ARG, "the index holds no minimizers: query sketches cannot be derived from it");
+  return qsketch_from_records(ctx, ix, ordinals, nq, queryIds);
+}
+
+QSketch *qsketch_from_records(Ctx *ctx, const Index *ix, const int32_t *ordinals, int32_t nq, const int32_t *queryIds)
+{
   std::vector<QuerySrc> srcs(nq);
   for (int i = 0; i < nq; i++) {
     const int32_t g = ordinals[i];
@@ -1108,9 +1115,7 @@ QSketch *qsketch_from_index(Ctx *ctx, const Index *ix, const int32_t *ordinals, 
     const int32_t c0 = g ? ix->seqsByFile[g - 1] : 0, c1 = ix->seqsByFile[g];
     srcs[i] = QuerySrc{nullptr, c1 - c0, ix->contigLen.data() + c0, c0};
   }
-  if (ix->M == 0 || !ix->validBits.p) fail(BANI_ERR_ARG, "the index holds no minimizers: query sketches cannot be derived from it");
-  const Index *hint = ix;
-  return qsketch_build(ctx, srcs, queryIds, hint);
+  return qsketch_build(ctx, srcs, queryIds, ix);
 }
 
 static QSketch *qsketch_build(Ctx *ctx, const std::vector<QuerySrc> &srcs, const int32_t *queryIds, const Index *hint)

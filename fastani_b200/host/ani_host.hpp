@@ -168,6 +168,26 @@ inline void upload_genomes(bani_ctx *ctx, const std::vector<const bani_host::Hos
   }
 }
 
+// The tables of a saved index file (bani_index_file_info; no device): per genome its contig count, length and cumulative
+// contig count, and every contig's length -- what a run plans its chunks and filters by --minFraction with
+struct IndexFileTables {
+  std::vector<int32_t> genomeContigs, seqsByFile, contigLen;
+  std::vector<uint64_t> genomeLen;
+};
+inline IndexFileTables indexFileTables(const std::string &path)
+{
+  int32_t nG = 0; uint64_t nC = 0;
+  check(bani_index_file_info(path.c_str(), nullptr, nullptr, nullptr, nullptr, &nG, &nC, nullptr, nullptr, nullptr, nullptr, nullptr, 0, nullptr, 0),
+        "bani_index_file_info");
+  IndexFileTables t;
+  t.genomeContigs.resize(std::max(nG, 1)); t.genomeLen.resize(std::max(nG, 1)); t.contigLen.resize(std::max<uint64_t>(nC, 1));
+  check(bani_index_file_info(path.c_str(), nullptr, nullptr, nullptr, nullptr, &nG, &nC, nullptr, t.genomeContigs.data(), t.genomeLen.data(),
+                             nullptr, nullptr, t.genomeContigs.size(), t.contigLen.data(), t.contigLen.size()), "bani_index_file_info");
+  t.genomeContigs.resize(nG); t.genomeLen.resize(nG); t.contigLen.resize(nC);
+  for (int32_t g = 0, c = 0; g < nG; g++) { c += t.genomeContigs[g]; t.seqsByFile.push_back(c); }
+  return t;
+}
+
 // ---------------------------------------------------------------------------------------- Sketch (HP1)
 class Sketch {
  public:
@@ -279,11 +299,11 @@ inline uint64_t genomeLength(const bani_host::HostGenome &g, int fragLen)
   return s;
 }
 
-// the same from a contig-length table (a reference genome known only through a loaded index)
-inline uint64_t genomeLength(const std::vector<skch::ContigInfo> &meta, int c0, int c1, int fragLen)
+// the same from a contig-length table (a reference genome known only through a saved index): contigs [c0, c1)
+inline uint64_t genomeLength(const std::vector<int32_t> &contigLen, int c0, int c1, int fragLen)
 {
   uint64_t s = 0;
-  for (int c = c0; c < c1; c++) if ((int64_t)meta[c].len >= fragLen) s += ((uint64_t)meta[c].len / (uint64_t)fragLen) * (uint64_t)fragLen;
+  for (int c = c0; c < c1; c++) if ((int64_t)contigLen[c] >= fragLen) s += ((uint64_t)contigLen[c] / (uint64_t)fragLen) * (uint64_t)fragLen;
   return s;
 }
 

@@ -52,7 +52,8 @@ static void usage(const char *prog, std::ostream &o)
        "                           deal, default) or block (contiguous ranges: list neighbours stay on one GPU)\n"
        "     --saveIndex <prefix>  write the reference sketches to <prefix>.meta + <prefix>.<shard>of<N>.idx after building them\n"
        "     --loadIndex <prefix>  take the references from a saved index instead of -r/--rl: no reference file is read or\n"
-       "                           sketched again; queries that are genomes of the index need no file either (1 GPU)\n"
+       "                           sketched again; queries that are genomes of the index need no file either (one shard).\n"
+       "                           Shard files are loaded in chunks that fit the device, on as many GPUs as are visible\n"
        "     --visualize           output mappings for visualization (<output>.visual)\n"
        "     --matrix              also output ANI values as lower triangular matrix (<output>.matrix)\n"
        "     -o, --output <value>  output file name\n"
@@ -212,7 +213,7 @@ int main(int argc, char **argv)
     }
     // a run that names its GPU count initialises only those devices (the driver's start-up cost grows with every visible GPU)
     {
-      const int want = loading ? meta.shards : parameters.gpus;
+      const int want = loading ? (parameters.gpus > 0 ? std::min(parameters.gpus, meta.shards) : meta.shards) : parameters.gpus;
       if (want > 0 && !getenv("CUDA_VISIBLE_DEVICES")) {
         std::string v; for (int g = 0; g < want; g++) v += (g ? "," : "") + std::to_string(g);
         setenv("CUDA_VISIBLE_DEVICES", v.c_str(), 0);
@@ -220,9 +221,11 @@ int main(int argc, char **argv)
     }
     int32_t nDev = 0;
     if (bani_device_count(&nDev) != BANI_OK || nDev == 0) throw std::runtime_error("no CUDA device available (this program has no CPU path)");
-    const int G = loading ? meta.shards : (parameters.gpus > 0 ? std::min(parameters.gpus, nDev) : nDev);
-    if (G > nDev) throw std::runtime_error("the saved index has " + std::to_string(G) + " shards but only " + std::to_string(nDev) + " GPU(s) are visible");
-    const auto shards = cgi::splitReferenceGenomes((int)parameters.refSequences.size(), G, parameters.blockPartition);
+    // S reference shards: one per GPU, or the saved index's shard files, of which GPU g takes g, g + G, ... in turn
+    const int visible = parameters.gpus > 0 ? std::min(parameters.gpus, (int)nDev) : (int)nDev;
+    const int G = loading ? std::min(visible, meta.shards) : visible;
+    const int S = loading ? meta.shards : G;
+    const auto shards = cgi::splitReferenceGenomes((int)parameters.refSequences.size(), S, parameters.blockPartition);
     // the contexts (CUDA context creation, stream set-up) come up while the reader threads parse and pack the files
     std::vector<bani_ctx *> ctxs(G, nullptr); std::vector<std::string> ctxErr(G);
     std::vector<std::thread> ctxThreads;
@@ -236,7 +239,7 @@ int main(int argc, char **argv)
     for (size_t j = 0; j < parameters.refSequences.size(); j++) refOrdinal.emplace(parameters.refSequences[j], (int)j);
     const char *hostCgiEnv = getenv("BANI_CLI_HOST_CGI");
     const bool hostCgi = parameters.visualize && hostCgiEnv && atoi(hostCgiEnv) != 0;     // per-query host computeCGI (test switch)
-    const bool deriveQueries = loading && G == 1 && !hostCgi;
+    const bool deriveQueries = loading && meta.shards == 1 && !hostCgi;
     auto derivable = [&](const std::string &q) { return deriveQueries && refOrdinal.count(q) > 0; };
     std::unordered_map<std::string, int> pathId; std::vector<std::string> paths;
     for (const auto &e : parameters.querySequences) if (!derivable(e) && !pathId.count(e)) { pathId[e] = (int)paths.size(); paths.push_back(e); }
@@ -263,66 +266,94 @@ int main(int argc, char **argv)
     for (int g = 0; g < G; g++) if (!ctxs[g]) throw std::runtime_error("bani_ctx_create: " + ctxErr[g]);
 
     std::vector<cgi::CGI_Results> finalResults;
-    std::vector<std::string> visual(G);
-    std::vector<char> sanity(G, 1); std::vector<float> ratioDiffs(G, 1.0f);
-    std::vector<std::vector<std::string>> savedContigNames(G);
+    std::vector<std::string> visual(S);
+    std::vector<char> sanity(S, 1); std::vector<float> ratioDiffs(S, 1.0f);
+    std::vector<std::vector<std::string>> savedContigNames(S);
     std::mutex mu; std::string err;
 
-    std::vector<std::vector<std::string>> chunkSanity(G);             // -s verdicts of chunked shards ("SPLIT g chunk c ...")
+    std::vector<std::vector<std::string>> chunkSanity(S);             // -s verdicts of chunked shards ("SPLIT s chunk c ...")
 
-    // A shard whose index does not fit the device at once.  Per query block: the block's queries are uploaded, hashed into
-    // sketches (no index to derive them from: every query is hashed) and their device genomes freed; then the shard's
-    // references are walked in chunks -- upload the planned genomes, build the longest prefix that fits the index budget
-    // (genomes it did not take stay uploaded for the next chunk), free the chunk's genomes, map, and hand the index and the
-    // cached blocks back before the next chunk.  Results carry shard-local reference ordinals, as those of one index would.
-    auto chunkedShard = [&](bani_ctx *ctx, int g, const std::vector<int> &shard, const std::vector<std::pair<int, int>> &chunks,
+    // One chunk's index against one query block's sketches: the -s verdict (reported for the first block), and the results
+    // with chunk-local reference ordinals moved to shard-local ones (+ first)
+    auto mapChunk = [&](bani_ctx *ctx, int s, int chunkNo, bool firstBlock, bani_index *ix, int first, const std::vector<bani_qsketch *> &sk,
+                        std::vector<cgi::CGI_Results> &local) {
+      float diff = 1.0f;
+      const bool sane = !parameters.sanityCheck || Sketch::indexSanityCheck(ix, parameters.maxRatioDiff, diff);
+      if (!sane && firstBlock) {
+        std::lock_guard<std::mutex> l(mu);
+        std::ostringstream m;                                       // the stream formatting of the per-split line
+        m << "ERROR :: SPLIT " << s << " chunk " << chunkNo << "'s ratio difference " << diff << " exceeds maximum thresholds.";
+        chunkSanity[s].push_back(m.str());
+      }
+      if (!sane) return;
+      bani_cgi_result *res = nullptr; uint64_t n = 0; bani_map_counters ctr;
+      check(bani_map_cgi_sketch(ctx, ix, sk.data(), (int32_t)sk.size(), &res, &n, &ctr), "bani_map_cgi_sketch");
+      for (uint64_t i = 0; i < n; i++)
+        local.push_back(cgi::CGI_Results{first + res[i].refGenomeId, res[i].qryGenomeId, res[i].countSeq, res[i].totalQueryFragments, res[i].identity});
+      bani_free(res);
+    };
+
+    // The sketches of query block [q0, q1): queries read from their files are hashed (their device genomes are freed
+    // again); with derive (a loaded one-shard index) the genomes of the index come from its file instead
+    auto blockSketches = [&](bani_ctx *ctx, int q0, int q1, int threads, const std::string &derivedFrom) {
+      std::vector<const bani_host::HostGenome *> qh; std::vector<int32_t> qid, dord, did;
+      for (int q = q0; q < q1; q++) {
+        const std::string &path = parameters.querySequences[q];
+        if (!derivedFrom.empty() && derivable(path)) { dord.push_back(refOrdinal.at(path)); did.push_back(q); }
+        else { qh.push_back(&genomes[pathId.at(path)]); qid.push_back(q); }
+      }
+      std::vector<bani_qsketch *> sk;
+      if (!qh.empty()) {
+        std::vector<std::unique_ptr<DeviceGenome>> dq;
+        upload_genomes(ctx, qh, dq, (size_t)1 << 28, threads);
+        std::vector<bani_genome *> hs; for (auto &d : dq) hs.push_back(d->h);
+        bani_qsketch *qsk = nullptr;
+        check(bani_qsketch_create(ctx, hs.data(), (int32_t)hs.size(), qid.data(), nullptr, &qsk), "bani_qsketch_create");
+        sk.push_back(qsk);
+      }
+      if (!dord.empty()) {
+        bani_qsketch *qsk = nullptr;
+        const int rc = bani_qsketch_from_index_file(ctx, derivedFrom.c_str(), dord.data(), (int32_t)dord.size(), did.data(), &qsk);
+        if (rc != BANI_OK) { for (auto *x : sk) bani_qsketch_destroy(x); check(rc, "bani_qsketch_from_index_file"); }
+        sk.push_back(qsk);
+      }
+      return sk;
+    };
+
+    // A shard whose index does not fit the device at once.  Per query block: the block's sketches are made; then the shard's
+    // references are walked in chunks -- built from uploads (the longest prefix of the planned genomes that fits the index
+    // budget: genomes it did not take stay uploaded for the next chunk) or loaded from the shard's saved file (the longest
+    // run from `first` that fits) -- each mapped, and the index and the cached blocks handed back before the next chunk.
+    // Results carry shard-local reference ordinals, as those of one index would.
+    auto chunkedShard = [&](bani_ctx *ctx, int s, const std::vector<int> &shard, const std::vector<std::pair<int, int>> &chunks,
                             const std::vector<std::pair<int, int>> &blocks, uint64_t indexBudget, std::vector<cgi::CGI_Results> &local) {
       const int threads = std::max(1, parameters.threads / G);
+      const std::string file = loading ? shardFile(parameters.loadIndex, s, S) : std::string();
       int chunkNo = 0;
       for (size_t b = 0; b < blocks.size(); b++) {
-        std::vector<const bani_host::HostGenome *> qh;
-        for (int q = blocks[b].first; q < blocks[b].second; q++) qh.push_back(&genomes[pathId.at(parameters.querySequences[q])]);
-        bani_qsketch *qsk = nullptr;
-        {
-          std::vector<std::unique_ptr<DeviceGenome>> dq;
-          upload_genomes(ctx, qh, dq, (size_t)1 << 28, threads);
-          std::vector<bani_genome *> hs; std::vector<int32_t> ids;
-          for (size_t i = 0; i < dq.size(); i++) { hs.push_back(dq[i]->h); ids.push_back(blocks[b].first + (int32_t)i); }
-          check(bani_qsketch_create(ctx, hs.data(), (int32_t)hs.size(), ids.data(), nullptr, &qsk), "bani_qsketch_create");
-        }
-        std::unique_ptr<bani_qsketch, void (*)(bani_qsketch *)> qskOwner(qsk, bani_qsketch_destroy);
+        std::vector<bani_qsketch *> sk = blockSketches(ctx, blocks[b].first, blocks[b].second, threads, deriveQueries ? file : std::string());
+        std::vector<std::unique_ptr<bani_qsketch, void (*)(bani_qsketch *)>> skOwner;
+        for (auto *x : sk) skOwner.emplace_back(x, bani_qsketch_destroy);
         std::vector<std::unique_ptr<DeviceGenome>> pending;
         int first = 0;
         size_t next = 0;
-        while (next < chunks.size() || !pending.empty()) {
-          if (pending.empty()) {
-            std::vector<const bani_host::HostGenome *> rh;
-            for (int i = chunks[next].first; i < chunks[next].second; i++) rh.push_back(&genomes[pathId.at(parameters.refSequences[shard[i]])]);
-            upload_genomes(ctx, rh, pending, (size_t)1 << 28, threads);
-            first = chunks[next].first;
-            next++;
-          }
-          std::vector<bani_genome *> hs; for (auto &d : pending) hs.push_back(d->h);
+        while (loading ? first < (int)shard.size() : (next < chunks.size() || !pending.empty())) {
           bani_index *ix = nullptr; int32_t taken = 0; uint64_t peak = 0;
-          check(bani_index_build_budget(ctx, hs.data(), (int32_t)hs.size(), indexBudget, &ix, &taken, &peak), "bani_index_build_budget");
+          if (loading) check(bani_index_load_budget(ctx, file.c_str(), first, indexBudget, &ix, &taken, &peak), "bani_index_load_budget");
+          else {
+            if (pending.empty()) {
+              std::vector<const bani_host::HostGenome *> rh;
+              for (int i = chunks[next].first; i < chunks[next].second; i++) rh.push_back(&genomes[pathId.at(parameters.refSequences[shard[i]])]);
+              upload_genomes(ctx, rh, pending, (size_t)1 << 28, threads);
+              first = chunks[next].first;
+              next++;
+            }
+            std::vector<bani_genome *> hs; for (auto &d : pending) hs.push_back(d->h);
+            check(bani_index_build_budget(ctx, hs.data(), (int32_t)hs.size(), indexBudget, &ix, &taken, &peak), "bani_index_build_budget");
+            pending.erase(pending.begin(), pending.begin() + taken);
+          }
           std::unique_ptr<bani_index, void (*)(bani_index *)> ixOwner(ix, bani_index_destroy);
-          pending.erase(pending.begin(), pending.begin() + taken);
-          float diff = 1.0f;
-          const bool sane = !parameters.sanityCheck || Sketch::indexSanityCheck(ix, parameters.maxRatioDiff, diff);
-          if (!sane && b == 0) {
-            std::lock_guard<std::mutex> l(mu);
-            std::ostringstream m;                                       // the stream formatting of the per-split line
-            m << "ERROR :: SPLIT " << g << " chunk " << chunkNo << "'s ratio difference " << diff << " exceeds maximum thresholds.";
-            chunkSanity[g].push_back(m.str());
-          }
-          if (sane) {
-            bani_cgi_result *res = nullptr; uint64_t n = 0; bani_map_counters ctr;
-            const bani_qsketch *one = qsk;
-            check(bani_map_cgi_sketch(ctx, ix, &one, 1, &res, &n, &ctr), "bani_map_cgi_sketch");
-            for (uint64_t i = 0; i < n; i++)
-              local.push_back(cgi::CGI_Results{first + res[i].refGenomeId, res[i].qryGenomeId, res[i].countSeq, res[i].totalQueryFragments, res[i].identity});
-            bani_free(res);
-          }
+          mapChunk(ctx, s, chunkNo, b == 0, ix, first, sk, local);
           ixOwner.reset();
           check(bani_ctx_trim(ctx), "bani_ctx_trim");
           first += taken;
@@ -331,173 +362,183 @@ int main(int argc, char **argv)
       }
     };
 
-    auto shardWork = [&](int g) {
-      try {
-        auto t1 = Clock::now();
-        bani_ctx *ctx = ctxs[g];
-        // ---- chunk plan: does the shard's index fit next to the query sketches and the mapping working set?  A saved index
-        //      is one index per shard, so a run that loads one has one chunk.
-        std::vector<std::pair<int, int>> chunks(1, {0, (int)shards[g].size()}), blocks(1, {0, (int)parameters.querySequences.size()});
-        uint64_t indexBudget = 0;
-        if (!loading) {
-          const auto &qs = parameters.querySequences;
-          std::vector<uint64_t> qlen(qs.size()), rlen; std::vector<int32_t> rcont;
-          for (size_t q = 0; q < qs.size(); q++) for (const auto &c : genomes[pathId.at(qs[q])].contigs) qlen[q] += c.len;
-          for (int j : shards[g]) {
-            const auto &h = genomes[pathId.at(parameters.refSequences[j])];
-            uint64_t len = 0; for (const auto &c : h.contigs) len += c.len;
-            rlen.push_back(len); rcont.push_back((int32_t)h.contigs.size());
-          }
-          std::vector<int32_t> cEnd(std::max<size_t>(rlen.size(), 1)), bEnd(std::max<size_t>(qs.size(), 1));
-          int32_t nc = 0, nb = 0;
-          check(bani_ctx_plan_run(ctx, 0, 0, rlen.data(), rcont.data(), (int32_t)rlen.size(), qlen.data(), nullptr, (int32_t)qs.size(),
-                                  cEnd.data(), &nc, bEnd.data(), &nb, &indexBudget), "bani_ctx_plan_run");
-          if (nc > 0) { chunks.clear(); for (int32_t c = 0, a = 0; c < nc; a = cEnd[c], c++) chunks.push_back({a, cEnd[c]}); }
-          if (nb > 0) { blocks.clear(); for (int32_t c = 0, a = 0; c < nb; a = bEnd[c], c++) blocks.push_back({a, bEnd[c]}); }
+    // reference shard s on GPU g (g == s unless a saved index has more shard files than the run has GPUs)
+    auto shardRun = [&](bani_ctx *ctx, int g, int s) {
+      auto t1 = Clock::now();
+      // ---- chunk plan: does the shard's index fit next to the query sketches and the mapping working set?
+      std::vector<std::pair<int, int>> chunks(1, {0, (int)shards[s].size()}), blocks(1, {0, (int)parameters.querySequences.size()});
+      uint64_t indexBudget = 0;
+      const auto &qs = parameters.querySequences;
+      std::vector<uint64_t> qlen(qs.size()), rlen; std::vector<int32_t> rcont;
+      if (loading) {                     // the saved shard file's tables: genome sizes for the plan and the --minFraction filter
+        const IndexFileTables t = indexFileTables(shardFile(parameters.loadIndex, s, S));
+        if (t.genomeLen.size() != shards[s].size())
+          throw std::runtime_error(shardFile(parameters.loadIndex, s, S) + " holds " + std::to_string(t.genomeLen.size()) + " genomes, " +
+                                   parameters.loadIndex + ".meta gives its shard " + std::to_string(shards[s].size()));
+        rlen = t.genomeLen; rcont = t.genomeContigs;
+        std::lock_guard<std::mutex> l(mu);
+        for (size_t i = 0; i < shards[s].size(); i++) {
+          const int c0 = i ? t.seqsByFile[i - 1] : 0;
+          genomeLengths.emplace(parameters.refSequences[shards[s][i]], cgi::genomeLength(t.contigLen, c0, t.seqsByFile[i], parameters.minReadLength));
         }
-        {
-          std::lock_guard<std::mutex> l(mu);
-          std::cerr << "INFO [GPU " << g << "], skch::main, reference chunks : " << chunks.size() << ", query blocks : " << blocks.size()
-                    << " (index budget " << indexBudget << " bytes)" << std::endl;
+      } else {
+        for (int j : shards[s]) {
+          const auto &h = genomes[pathId.at(parameters.refSequences[j])];
+          uint64_t len = 0; for (const auto &c : h.contigs) len += c.len;
+          rlen.push_back(len); rcont.push_back((int32_t)h.contigs.size());
         }
-        if (chunks.size() > 1 || blocks.size() > 1) {
-          if (parameters.visualize)
-            throw std::runtime_error("--visualize needs the reference shard of a GPU in one index, this run needs " + std::to_string(chunks.size()) +
-                                     " chunk(s) and " + std::to_string(blocks.size()) + " query block(s) on GPU " + std::to_string(g) + ": use more GPUs or fewer references");
-          if (!parameters.saveIndex.empty())
-            throw std::runtime_error("--saveIndex writes one index per GPU, this run needs " + std::to_string(chunks.size()) + " chunk(s) and " +
-                                     std::to_string(blocks.size()) + " query block(s) on GPU " + std::to_string(g) + ": use more GPUs or fewer references");
-          std::vector<cgi::CGI_Results> local;
-          chunkedShard(ctx, g, shards[g], chunks, blocks, indexBudget, local);
-          if (g == 0) std::cerr << "INFO [GPU 0], skch::main, Time spent sketching and mapping in chunks : "
-                                << std::chrono::duration<double>(Clock::now() - t1).count() << " sec" << std::endl;
-          cgi::correctRefGenomeIds(local, g, G, (int)parameters.refSequences.size(), parameters.blockPartition);
-          std::lock_guard<std::mutex> l(mu);
-          finalResults.insert(finalResults.end(), local.begin(), local.end());
-        } else {
-          // genomes this device needs: its reference shard (unless loaded) and every query that has to be read, each file once
-          std::vector<int> need; std::unordered_map<int, int> slot;
-          auto want = [&](const std::string &path) { const int id = pathId.at(path); if (!slot.count(id)) { slot[id] = (int)need.size(); need.push_back(id); } return slot[id]; };
-          std::vector<int> refSlot, qrySlot;                              // qrySlot: -1 = derived from the index
-          if (!loading) for (int j : shards[g]) refSlot.push_back(want(parameters.refSequences[j]));
-          for (const auto &q : parameters.querySequences) qrySlot.push_back(derivable(q) ? -1 : want(q));
-          std::vector<const bani_host::HostGenome *> hs; for (int id : need) hs.push_back(&genomes[id]);
-          std::vector<std::unique_ptr<DeviceGenome>> dev;
-          upload_genomes(ctx, hs, dev, (size_t)1 << 28, std::max(1, parameters.threads / G));
-          std::vector<std::string> shardRefNames;
-          for (int j : shards[g]) shardRefNames.push_back(parameters.refSequences[j]);
+      }
+      for (size_t q = 0; q < qs.size(); q++) {
+        if (derivable(qs[q])) { qlen[q] = rlen[refOrdinal.at(qs[q])]; continue; }      // one shard: its ordinal in the file
+        for (const auto &c : genomes[pathId.at(qs[q])].contigs) qlen[q] += c.len;
+      }
+      std::vector<int32_t> cEnd(std::max<size_t>(rlen.size(), 1)), bEnd(std::max<size_t>(qs.size(), 1));
+      int32_t nc = 0, nb = 0;
+      check(bani_ctx_plan_run(ctx, 0, 0, rlen.data(), rcont.data(), (int32_t)rlen.size(), qlen.data(), nullptr, (int32_t)qs.size(),
+                              cEnd.data(), &nc, bEnd.data(), &nb, &indexBudget), "bani_ctx_plan_run");
+      if (nc > 0) { chunks.clear(); for (int32_t c = 0, a = 0; c < nc; a = cEnd[c], c++) chunks.push_back({a, cEnd[c]}); }
+      if (nb > 0) { blocks.clear(); for (int32_t c = 0, a = 0; c < nb; a = bEnd[c], c++) blocks.push_back({a, bEnd[c]}); }
+      {
+        std::lock_guard<std::mutex> l(mu);
+        std::cerr << "INFO [GPU " << g << "], skch::main, " << (loading ? "shard file " + std::to_string(s) + ", " : std::string())
+                  << "reference chunks : " << chunks.size() << ", query blocks : " << blocks.size() << " (index budget " << indexBudget << " bytes)" << std::endl;
+      }
+      if (chunks.size() > 1 || blocks.size() > 1) {
+        if (parameters.visualize)
+          throw std::runtime_error("--visualize needs the reference shard of a GPU in one index, this run needs " + std::to_string(chunks.size()) +
+                                   " chunk(s) and " + std::to_string(blocks.size()) + " query block(s) on GPU " + std::to_string(g) + ": use more GPUs or fewer references");
+        if (!parameters.saveIndex.empty())
+          throw std::runtime_error("--saveIndex writes one index per GPU, this run needs " + std::to_string(chunks.size()) + " chunk(s) and " +
+                                   std::to_string(blocks.size()) + " query block(s) on GPU " + std::to_string(g) + ": use more GPUs or fewer references");
+        std::vector<cgi::CGI_Results> local;
+        chunkedShard(ctx, s, shards[s], chunks, blocks, indexBudget, local);
+        if (g == 0) std::cerr << "INFO [GPU 0], skch::main, Time spent " << (loading ? "loading" : "sketching") << " and mapping in chunks : "
+                              << std::chrono::duration<double>(Clock::now() - t1).count() << " sec" << std::endl;
+        cgi::correctRefGenomeIds(local, s, S, (int)parameters.refSequences.size(), parameters.blockPartition);
+        std::lock_guard<std::mutex> l(mu);
+        finalResults.insert(finalResults.end(), local.begin(), local.end());
+        return;
+      }
+      // genomes this device needs: its reference shard (unless loaded) and every query that has to be read, each file once
+      std::vector<int> need; std::unordered_map<int, int> slot;
+      auto want = [&](const std::string &path) { const int id = pathId.at(path); if (!slot.count(id)) { slot[id] = (int)need.size(); need.push_back(id); } return slot[id]; };
+      std::vector<int> refSlot, qrySlot;                              // qrySlot: -1 = derived from the index
+      if (!loading) for (int j : shards[s]) refSlot.push_back(want(parameters.refSequences[j]));
+      for (const auto &q : parameters.querySequences) qrySlot.push_back(derivable(q) ? -1 : want(q));
+      std::vector<const bani_host::HostGenome *> hs; for (int id : need) hs.push_back(&genomes[id]);
+      std::vector<std::unique_ptr<DeviceGenome>> dev;
+      upload_genomes(ctx, hs, dev, (size_t)1 << 28, std::max(1, parameters.threads / G));
+      std::vector<std::string> shardRefNames;
+      for (int j : shards[s]) shardRefNames.push_back(parameters.refSequences[j]);
 
-          std::unique_ptr<Sketch> referSketchP;                           // HP1, or the cache
-          if (loading) referSketchP.reset(new Sketch(ctx, parameters, shardFile(parameters.loadIndex, g, G), meta.contigNames[g]));
-          else {
-            std::vector<const DeviceGenome *> refs;
-            for (int sl : refSlot) refs.push_back(dev[sl].get());
-            referSketchP.reset(new Sketch(ctx, parameters, refs));
+      std::unique_ptr<Sketch> referSketchP;                           // HP1, or the cache
+      if (loading) referSketchP.reset(new Sketch(ctx, parameters, shardFile(parameters.loadIndex, s, S), meta.contigNames[s]));
+      else {
+        std::vector<const DeviceGenome *> refs;
+        for (int sl : refSlot) refs.push_back(dev[sl].get());
+        referSketchP.reset(new Sketch(ctx, parameters, refs));
+      }
+      Sketch &referSketch = *referSketchP;
+      if (g == 0) std::cerr << "INFO [GPU 0], skch::main, Time spent " << (loading ? "loading" : "sketching") << " the reference : "
+                            << std::chrono::duration<double>(Clock::now() - t1).count() << " sec" << std::endl;
+      if (!parameters.saveIndex.empty()) {
+        referSketch.save(shardFile(parameters.saveIndex, s, S));
+        for (const auto &c : referSketch.metadata) savedContigNames[s].push_back(c.name);
+      }
+      std::vector<cgi::CGI_Results> local;
+      sanity[s] = referSketch.sanityCheck(parameters.maxRatioDiff); ratioDiffs[s] = referSketch.getRatioDifference();
+      if (sanity[s]) {
+        t1 = Clock::now();
+        if (hostCgi) {
+          std::ostringstream vis;
+          for (size_t q = 0; q < qrySlot.size(); q++) {
+            MappingResultsVector_t mapResults; uint64_t totalQueryFragments = 0;
+            Map mapper(ctx, parameters, referSketch, *dev[qrySlot[q]], totalQueryFragments,
+                       std::bind(Map::insertL2ResultsToVec, std::ref(mapResults), std::placeholders::_1));     // HP2
+            cgi::computeCGI(parameters, mapResults, mapper, referSketch, totalQueryFragments, q, parameters.querySequences[q],
+                            shardRefNames, &vis, local);
           }
-          Sketch &referSketch = *referSketchP;
-          if (g == 0) std::cerr << "INFO [GPU 0], skch::main, Time spent " << (loading ? "loading" : "sketching") << " the reference : "
-                                << std::chrono::duration<double>(Clock::now() - t1).count() << " sec" << std::endl;
-          if (!parameters.saveIndex.empty()) {
-            referSketch.save(shardFile(parameters.saveIndex, g, G));
-            for (const auto &c : referSketch.metadata) savedContigNames[g].push_back(c.name);
+          visual[s] = vis.str();
+        } else {
+          // HP2 + reduction for all queries: one sketch object for the queries that were read, one for those derived
+          std::vector<bani_genome *> qh; std::vector<int32_t> qid, dord, did;
+          for (size_t q = 0; q < qrySlot.size(); q++) {
+            if (qrySlot[q] >= 0) { qh.push_back(dev[qrySlot[q]]->h); qid.push_back((int32_t)q); }
+            else { dord.push_back(refOrdinal.at(parameters.querySequences[q])); did.push_back((int32_t)q); }
           }
-          if (loading) {                                                  // lengths of the shard's genomes for the --minFraction filter
-            std::lock_guard<std::mutex> l(mu);
-            for (size_t i = 0; i < shards[g].size(); i++) {
-              const int c0 = i ? referSketch.sequencesByFileInfo[i - 1] : 0, c1 = referSketch.sequencesByFileInfo[i];
-              genomeLengths.emplace(shardRefNames[i], cgi::genomeLength(referSketch.metadata, c0, c1, parameters.minReadLength));
+          std::vector<bani_qsketch *> sk;
+          if (!qh.empty()) { bani_qsketch *x = nullptr; check(bani_qsketch_create(ctx, qh.data(), (int32_t)qh.size(), qid.data(), referSketch.handle(), &x), "bani_qsketch_create"); sk.push_back(x); }
+          if (!dord.empty()) { bani_qsketch *x = nullptr; check(bani_qsketch_from_index(ctx, referSketch.handle(), dord.data(), (int32_t)dord.size(), did.data(), &x), "bani_qsketch_from_index"); sk.push_back(x); }
+          bani_cgi_result *res = nullptr; uint64_t n = 0; bani_map_counters ctr;
+          bani_frag_mapping *frags = nullptr; uint64_t nf = 0;
+          const int rc = parameters.visualize                                                                  // HP2 + reduction
+            ? bani_map_cgi_sketch_frags(ctx, referSketch.handle(), sk.data(), (int32_t)sk.size(), &res, &n, &frags, &nf, &ctr)
+            : bani_map_cgi_sketch(ctx, referSketch.handle(), sk.data(), (int32_t)sk.size(), &res, &n, &ctr);
+          for (auto *x : sk) bani_qsketch_destroy(x);
+          check(rc, parameters.visualize ? "bani_map_cgi_sketch_frags" : "bani_map_cgi_sketch");
+          for (uint64_t i = 0; i < n; i++)
+            local.push_back(cgi::CGI_Results{res[i].refGenomeId, res[i].qryGenomeId, res[i].countSeq, res[i].totalQueryFragments, res[i].identity});
+          bani_free(res);
+          if (parameters.visualize) {
+            // frags come per sketch (queries read, then queries derived): .visual lines go in query-list order.  The
+            // frags of one query are contiguous and in bin order, so a stable sort by query keeps that order.
+            std::stable_sort(frags, frags + nf, [](const bani_frag_mapping &a, const bani_frag_mapping &b) { return a.qryGenomeId < b.qryGenomeId; });
+            std::vector<skch::offset_t> refLens;
+            for (const auto &c : referSketch.metadata) refLens.push_back(c.len);
+            const std::vector<int64_t> refOff = cgi::offsetAdder(refLens);
+            std::ostringstream vis;
+            for (uint64_t i = 0; i < nf;) {
+              const int32_t q = frags[i].qryGenomeId;
+              uint64_t j = i;
+              while (j < nf && frags[j].qryGenomeId == q) j++;
+              // Map::metadata of the query: from its file, or (derived query) from its contigs in the index
+              std::vector<skch::offset_t> qLens;
+              if (qrySlot[q] >= 0) {
+                for (const auto &c : dev[qrySlot[q]]->host->contigs) appendFragmentLengths(parameters, (offset_t)c.len, qLens);
+              } else {
+                const int o = refOrdinal.at(parameters.querySequences[q]);
+                const int c0 = o ? referSketch.sequencesByFileInfo[o - 1] : 0, c1 = referSketch.sequencesByFileInfo[o];
+                for (int c = c0; c < c1; c++) appendFragmentLengths(parameters, referSketch.metadata[c].len, qLens);
+              }
+              cgi::outputVisualizationFile(parameters, frags + i, j - i, cgi::offsetAdder(qLens), refOff, referSketch,
+                                           parameters.querySequences[q], shardRefNames, vis);
+              i = j;
             }
+            visual[s] = vis.str();
           }
-          std::vector<cgi::CGI_Results> local;
-          sanity[g] = referSketch.sanityCheck(parameters.maxRatioDiff); ratioDiffs[g] = referSketch.getRatioDifference();
-          if (sanity[g]) {
-            t1 = Clock::now();
-            if (hostCgi) {
-              std::ostringstream vis;
-              for (size_t q = 0; q < qrySlot.size(); q++) {
-                MappingResultsVector_t mapResults; uint64_t totalQueryFragments = 0;
-                Map mapper(ctx, parameters, referSketch, *dev[qrySlot[q]], totalQueryFragments,
-                           std::bind(Map::insertL2ResultsToVec, std::ref(mapResults), std::placeholders::_1));     // HP2
-                cgi::computeCGI(parameters, mapResults, mapper, referSketch, totalQueryFragments, q, parameters.querySequences[q],
-                                shardRefNames, &vis, local);
-              }
-              visual[g] = vis.str();
-            } else {
-              // HP2 + reduction for all queries: one sketch object for the queries that were read, one for those derived
-              std::vector<bani_genome *> qh; std::vector<int32_t> qid, dord, did;
-              for (size_t q = 0; q < qrySlot.size(); q++) {
-                if (qrySlot[q] >= 0) { qh.push_back(dev[qrySlot[q]]->h); qid.push_back((int32_t)q); }
-                else { dord.push_back(refOrdinal.at(parameters.querySequences[q])); did.push_back((int32_t)q); }
-              }
-              std::vector<bani_qsketch *> sk;
-              if (!qh.empty()) { bani_qsketch *s = nullptr; check(bani_qsketch_create(ctx, qh.data(), (int32_t)qh.size(), qid.data(), referSketch.handle(), &s), "bani_qsketch_create"); sk.push_back(s); }
-              if (!dord.empty()) { bani_qsketch *s = nullptr; check(bani_qsketch_from_index(ctx, referSketch.handle(), dord.data(), (int32_t)dord.size(), did.data(), &s), "bani_qsketch_from_index"); sk.push_back(s); }
-              bani_cgi_result *res = nullptr; uint64_t n = 0; bani_map_counters ctr;
-              bani_frag_mapping *frags = nullptr; uint64_t nf = 0;
-              const int rc = parameters.visualize                                                                  // HP2 + reduction
-                ? bani_map_cgi_sketch_frags(ctx, referSketch.handle(), sk.data(), (int32_t)sk.size(), &res, &n, &frags, &nf, &ctr)
-                : bani_map_cgi_sketch(ctx, referSketch.handle(), sk.data(), (int32_t)sk.size(), &res, &n, &ctr);
-              for (auto *s : sk) bani_qsketch_destroy(s);
-              check(rc, parameters.visualize ? "bani_map_cgi_sketch_frags" : "bani_map_cgi_sketch");
-              for (uint64_t i = 0; i < n; i++)
-                local.push_back(cgi::CGI_Results{res[i].refGenomeId, res[i].qryGenomeId, res[i].countSeq, res[i].totalQueryFragments, res[i].identity});
-              bani_free(res);
-              if (parameters.visualize) {
-                // frags come per sketch (queries read, then queries derived): .visual lines go in query-list order.  The
-                // frags of one query are contiguous and in bin order, so a stable sort by query keeps that order.
-                std::stable_sort(frags, frags + nf, [](const bani_frag_mapping &a, const bani_frag_mapping &b) { return a.qryGenomeId < b.qryGenomeId; });
-                std::vector<skch::offset_t> refLens;
-                for (const auto &c : referSketch.metadata) refLens.push_back(c.len);
-                const std::vector<int64_t> refOff = cgi::offsetAdder(refLens);
-                std::ostringstream vis;
-                for (uint64_t i = 0; i < nf;) {
-                  const int32_t q = frags[i].qryGenomeId;
-                  uint64_t j = i;
-                  while (j < nf && frags[j].qryGenomeId == q) j++;
-                  // Map::metadata of the query: from its file, or (derived query) from its contigs in the index
-                  std::vector<skch::offset_t> qLens;
-                  if (qrySlot[q] >= 0) {
-                    for (const auto &c : dev[qrySlot[q]]->host->contigs) appendFragmentLengths(parameters, (offset_t)c.len, qLens);
-                  } else {
-                    const int o = refOrdinal.at(parameters.querySequences[q]);
-                    const int c0 = o ? referSketch.sequencesByFileInfo[o - 1] : 0, c1 = referSketch.sequencesByFileInfo[o];
-                    for (int c = c0; c < c1; c++) appendFragmentLengths(parameters, referSketch.metadata[c].len, qLens);
-                  }
-                  cgi::outputVisualizationFile(parameters, frags + i, j - i, cgi::offsetAdder(qLens), refOff, referSketch,
-                                               parameters.querySequences[q], shardRefNames, vis);
-                  i = j;
-                }
-                visual[g] = vis.str();
-              }
-              bani_free(frags);
-            }
-            if (g == 0) std::cerr << "INFO [GPU 0], skch::main, Time spent mapping " << qrySlot.size() << " query genome(s) : "
-                                  << std::chrono::duration<double>(Clock::now() - t1).count() << " sec" << std::endl;
-          }
-          cgi::correctRefGenomeIds(local, g, G, (int)parameters.refSequences.size(), parameters.blockPartition);
-          std::lock_guard<std::mutex> l(mu);
-          finalResults.insert(finalResults.end(), local.begin(), local.end());
+          bani_free(frags);
         }
-        if (getenv("BANI_CLI_FULL_TEARDOWN")) bani_ctx_destroy(ctx);      // otherwise the process exit returns the device memory (faster)
+        if (g == 0) std::cerr << "INFO [GPU 0], skch::main, Time spent mapping " << qrySlot.size() << " query genome(s) : "
+                              << std::chrono::duration<double>(Clock::now() - t1).count() << " sec" << std::endl;
+      }
+      cgi::correctRefGenomeIds(local, s, S, (int)parameters.refSequences.size(), parameters.blockPartition);
+      std::lock_guard<std::mutex> l(mu);
+      finalResults.insert(finalResults.end(), local.begin(), local.end());
+    };
+
+    auto gpuWork = [&](int g) {
+      try {
+        for (int s = g; s < S; s += G) shardRun(ctxs[g], g, s);
+        if (getenv("BANI_CLI_FULL_TEARDOWN")) bani_ctx_destroy(ctxs[g]);      // otherwise the process exit returns the device memory (faster)
       } catch (const std::exception &e) { std::lock_guard<std::mutex> l(mu); err = e.what(); }
     };
     {
       std::vector<std::thread> th;
-      for (int g = 0; g < G; g++) th.emplace_back(shardWork, g);
+      for (int g = 0; g < G; g++) th.emplace_back(gpuWork, g);
       for (auto &t : th) t.join();
     }
     if (!err.empty()) throw std::runtime_error(err);
-    if (!parameters.saveIndex.empty()) writeMeta(parameters.saveIndex, parameters, G, savedContigNames);
-    for (int g = 0; g < G; g++) {
-      if (!sanity[g]) std::cerr << "ERROR :: SPLIT " << g << "'s ratio difference " << ratioDiffs[g] << " exceeds maximum thresholds." << std::endl;
-      for (const auto &m : chunkSanity[g]) std::cerr << m << std::endl;
+    if (!parameters.saveIndex.empty()) writeMeta(parameters.saveIndex, parameters, S, savedContigNames);
+    for (int s = 0; s < S; s++) {
+      if (!sanity[s]) std::cerr << "ERROR :: SPLIT " << s << "'s ratio difference " << ratioDiffs[s] << " exceeds maximum thresholds." << std::endl;
+      for (const auto &m : chunkSanity[s]) std::cerr << m << std::endl;
     }
     // a query derived from the index has the length its reference twin has
     for (const auto &q : parameters.querySequences) if (!genomeLengths.count(q)) throw std::runtime_error("no length known for " + q);
 
     cgi::outputCGI(parameters, genomeLengths, finalResults, fileName);
     if (parameters.matrixOutput) cgi::outputPhylip(parameters, genomeLengths, finalResults, fileName);
-    if (parameters.visualize) { std::ofstream o(fileName + ".visual"); for (int g = 0; g < G; g++) o << visual[g]; }
+    if (parameters.visualize) { std::ofstream o(fileName + ".visual"); for (int s = 0; s < S; s++) o << visual[s]; }
     std::cerr << "INFO, skch::main, Total time : " << std::chrono::duration<double>(Clock::now() - tStart).count() << " sec" << std::endl;
   } catch (const std::exception &e) {
     std::cerr << "ERROR, " << e.what() << std::endl;

@@ -283,7 +283,7 @@ BANI_API int  bani_index_lookup(bani_ctx *ctx, const bani_index *ix, uint32_t ha
 
 /* ---- on-disk sketch cache (the reference has none: scripts/splitDatabase.sh + README.md:104-106 re-sketch every
  * reference in every run).  bani_index_save writes what only the sketch launch can produce -- position-ordered
- * (hash, wpos) records, contig table, validity bitmap, parameters, checksum -- as one flat file; bani_index_load reads
+ * (hash, wpos) records, contig table, validity bitmap, parameters, checksums -- as one flat file; bani_index_load reads
  * it back on a context with the SAME k / window / fragLen (anything else is refused, like an in-memory mismatch) and
  * rebuilds the lookup side on the GPU.  Host metadata (genome paths, contig names) is the caller's to store. */
 BANI_API int  bani_index_save(bani_ctx *ctx, const bani_index *ix, const char *path);
@@ -292,6 +292,32 @@ BANI_API int  bani_index_load(bani_ctx *ctx, const char *path, bani_index **out)
  * genome (== Sketch::sequencesByFileInfo, winSketch.hpp:75; cap >= n_genomes): what a host needs to rebuild
  * Sketch::metadata lengths and computeGenomeLengths (computeCoreIdentity.hpp:48-92) for a loaded index. */
 BANI_API int  bani_index_contigs(const bani_index *ix, int32_t *contig_len, uint64_t cap_contigs, int32_t *seqs_by_file, uint64_t cap_genomes);
+
+/* ---- saved index files read in ranges: a file need not fit the device, nor was it necessarily saved on as many GPUs.
+ * Files are written in version 3 (bani_index_save): besides the whole-file checksum they hold a checksum of the header and
+ * contig tables and one per genome (its records and validity bitmap words), so that a run of genomes can be read and
+ * verified alone.  Version 2 files (whole-file checksum only) still load whole with bani_index_load; the two calls that
+ * read ranges refuse them with BANI_ERR_ARG (save the index again).
+ *
+ * bani_index_file_info: the header and tables of a saved index file, checked as bani_index_load checks them (version 3:
+ * against their checksum).  Host only: no context, no device.  Every output is optional (NULL skips it).  Per genome
+ * (cap_genomes >= *n_genomes): genome_contigs its contig count, genome_len its total length in bases, genome_records its
+ * minimizer count, genome_bits its validity bitmap bits (its contig lengths, each rounded up to 32).  contig_len: every
+ * contig's length in seqId order (cap_contigs >= *n_contigs).  Call once without arrays for the counts.  What a host
+ * needs to plan chunks (bani_plan_run, bani_index_footprint) and the --minFraction genome lengths without loading. */
+BANI_API int  bani_index_file_info(const char *path, int32_t *version, int32_t *k, int32_t *w, int32_t *frag_len, int32_t *n_genomes,
+                                   uint64_t *n_contigs, uint64_t *n_minimizers, int32_t *genome_contigs, uint64_t *genome_len,
+                                   uint64_t *genome_records, uint64_t *genome_bits, uint64_t cap_genomes, int32_t *contig_len,
+                                   uint64_t cap_contigs);
+/* The loading twin of bani_index_build_budget: the index of the longest run of genomes [first_genome, first_genome +
+ * *n_taken) of a saved file whose load fits max_bytes of device memory (bani_index_footprint of the run's exact minimizer,
+ * contig and bitmap counts, with no sketch staging), at least one genome; a first genome that does not fit alone gives
+ * BANI_ERR_LIMIT (never a failed allocation).  Only that run's contig tables, records and bitmap words are read, each
+ * checked against its checksum.  The index equals byte for byte bani_index_build's of exactly those genomes (minimizers,
+ * stats, contigs, validity bitmap, mappings, derived query sketches).  *peak_bytes (optional): the most device memory the
+ * call held above what was held on entry.  Same k / window / fragLen as the context, as for bani_index_load. */
+BANI_API int  bani_index_load_budget(bani_ctx *ctx, const char *path, int32_t first_genome, uint64_t max_bytes, bani_index **out,
+                                     int32_t *n_taken, uint64_t *peak_bytes);
 
 /* ---- HP2: query mapping ---------------------------------------------------
  * Map::mapQuery (computeMap.hpp:112-196) for one query genome: every mapping the
@@ -326,6 +352,11 @@ BANI_API int  bani_qsketch_create(bani_ctx *ctx, bani_genome *const *queries, in
  * loaded from disk is also the query side of an all-vs-all run. */
 BANI_API int  bani_qsketch_from_index(bani_ctx *ctx, const bani_index *ix, const int32_t *genome_ordinals, int32_t n_queries,
                                       const int32_t *query_ids, bani_qsketch **out);
+/* bani_qsketch_from_index for genomes of a saved file (version 3), by genome ordinal, without loading the index: only those genomes'
+ * records, bitmap words and contig tables are read, each checked against its genome's checksum.  bani_qsketch_info and
+ * every mapping result equal those of bani_qsketch_from_index on the whole loaded file. */
+BANI_API int  bani_qsketch_from_index_file(bani_ctx *ctx, const char *path, const int32_t *genome_ordinals, int32_t n_queries,
+                                           const int32_t *query_ids, bani_qsketch **out);
 BANI_API void bani_qsketch_destroy(bani_qsketch *qs);
 BANI_API int  bani_qsketch_info(const bani_qsketch *qs, int32_t *n_queries, uint64_t *n_fragments, uint64_t *n_hashes,
                                 uint64_t *export_bytes);
