@@ -226,7 +226,7 @@ class Context:
     def set_flag(self, name, value):
         """bani_ctx_set_flag: "sketch_reuse", "max_hits_per_piece", "frag_l1_max", "l2e_buckets", "l2_stage",
         "upload_group_words", "frags_per_piece", "event_bytes_per_piece", "cgi_table_queries", "l2_fast", "count_paths",
-        "index_bytes_budget", "query_sketch_budget"."""
+        "cgi_sparse" (-1 chosen per piece, 0 dense, 1 sparse identity reduction), "index_bytes_budget", "query_sketch_budget"."""
         _check(self.lib.bani_ctx_set_flag(self.h, name.encode(), int(value)))
 
     def path_counts(self):

@@ -18,7 +18,7 @@ const char *const PATH_NAMES[NPATH] = {
   "lookup.walk_saturated", "lookup.walk_full_bucket",
   "l2.events_nt64", "l2.events_nt128", "l2.events_nt256", "l2.dir1024", "l2.dir4096", "l2.staged", "l2.direct",
   "l2.exact_at_bounds", "l2.exact_total",
-  "piece.mapped", "piece.split_hits", "piece.split_events", "cgi.passes"};
+  "piece.mapped", "piece.split_hits", "piece.split_events", "cgi.passes", "cgi.sparse"};
 }
 
 using namespace bani;
@@ -124,6 +124,13 @@ int bani_ctx_create(int device, const bani_params *p, bani_ctx **out)
     if (const char *e = getenv("BANI_L2_STAGE")) f.l2Stage = atoi(e) != 0;
     if (const char *e = getenv("BANI_TRACE")) f.trace = atoi(e) != 0;
     if (const char *e = getenv("BANI_L2E_BUCKETS")) { const int v = atoi(e); if (v == 1024 || v == 4096) f.l2eBuckets = v; }
+    if (const char *e = getenv("BANI_CGI_SPARSE")) {
+      const std::string v(e);
+      if (v == "-1") f.cgiSparse = -1;
+      else if (v == "0") f.cgiSparse = 0;
+      else if (v == "1") f.cgiSparse = 1;
+      else fail(BANI_ERR_ARG, "BANI_CGI_SPARSE=%s is not -1 (chosen per piece), 0 (dense) or 1 (sparse)", e);
+    }
     uint64_t b = 0;
     if (const char *e = getenv("BANI_INDEX_BUDGET")) {
       if (!parse_byte_count(e, &b)) fail(BANI_ERR_ARG, "BANI_INDEX_BUDGET=%s is not a byte count (digits, optionally followed by K, M or G)", e);
@@ -191,6 +198,7 @@ int bani_ctx_set_flag(bani_ctx *ctx, const char *name, int64_t value)
   else if (n == "cgi_table_queries") { if (value < 0) fail(BANI_ERR_ARG, "cgi_table_queries must not be negative"); f.cgiTableQueries = value; }
   else if (n == "l2_fast") f.l2Fast = value != 0;
   else if (n == "count_paths") f.countPaths = value != 0;
+  else if (n == "cgi_sparse") { if (value < -1 || value > 1) fail(BANI_ERR_ARG, "cgi_sparse must be -1, 0 or 1"); f.cgiSparse = (int)value; }
   else if (n == "index_bytes_budget") { if (value < 0) fail(BANI_ERR_ARG, "index_bytes_budget must not be negative"); f.indexBytesBudget = (unsigned long long)value; }
   else if (n == "query_sketch_budget") { if (value < 0) fail(BANI_ERR_ARG, "query_sketch_budget must not be negative"); f.querySketchBudget = (unsigned long long)value; }
   else fail(BANI_ERR_ARG, "unknown flag '%s'", name);

@@ -200,7 +200,8 @@ struct View {
 };
 
 // Run-time switches of a context (bani_ctx_set_flag); the defaults can also be set through the environment
-// (BANI_NO_SKETCH_REUSE, BANI_MAX_HITS_PER_PIECE, BANI_FRAG_L1_MAX, BANI_L2E_BUCKETS, BANI_L2_STAGE, BANI_TRACE), read when the context is created.
+// (BANI_NO_SKETCH_REUSE, BANI_MAX_HITS_PER_PIECE, BANI_FRAG_L1_MAX, BANI_L2E_BUCKETS, BANI_L2_STAGE, BANI_TRACE, BANI_CGI_SPARSE),
+// read when the context is created.
 struct CtxFlags {
   int sketchReuse = 1;                        // stage A': fragment sketches of index members are read from the index
   long long maxHitsPerPiece = 3ll << 29;      // a piece that gathers more index hits is split at a query boundary
@@ -218,6 +219,7 @@ struct CtxFlags {
   long long cgiTableQueries = 0;              // queries per pass of the identity reduction; 0 = as many as 3 GiB of bin table hold
   int l2Fast = 1;                             // 0: every L2 candidate goes to the exact kernel (l2_kernel)
   int countPaths = 0;                         // 1: count which branch of the mapping path ran (bani_ctx_path_counts)
+  int cgiSparse = -1;                         // stage H per piece: -1 chosen from the piece's size, 0 dense tables, 1 sparse rows
   // Budgets of a run that builds its references in chunks (bani_ctx_plan_run); results never depend on them.
   unsigned long long indexBytesBudget = 0;    // build peak of one chunk's index; 0 = derived from device memory
   unsigned long long querySketchBudget = 0;   // query sketches resident at once; 0 = derived from device memory
@@ -225,14 +227,15 @@ struct CtxFlags {
 
 // Branches of the mapping path, counted when CtxFlags::countPaths is set (names: capi.cu, bani_ctx_path_counts).  What a
 // counter counts: fragments per L1 size class; probes that walked the sorted keys; L2 candidates with window events per
-// event-kernel variant; candidates left to the exact kernel after the bounds pass and in total; pieces and passes.
+// event-kernel variant; candidates left to the exact kernel after the bounds pass and in total; pieces and passes;
+// pieces whose identity reduction took the sparse path (cgi.passes counts dense passes only).
 // The per-piece counters (everything but piece.split_*) are those of the pieces that were mapped, not of those split.
 enum PathId {
   P_L1_CLASS0 = 0, P_L1_DEVICE_WIDE = 13,                    // 13 == FRAG_NCLASS
   P_LOOKUP_WALK_SATURATED, P_LOOKUP_WALK_FULL_BUCKET,
   P_L2_EVENTS_NT64, P_L2_EVENTS_NT128, P_L2_EVENTS_NT256, P_L2_DIR1024, P_L2_DIR4096, P_L2_STAGED, P_L2_DIRECT,
   P_L2_EXACT_AT_BOUNDS, P_L2_EXACT_TOTAL,
-  P_PIECE_MAPPED, P_PIECE_SPLIT_HITS, P_PIECE_SPLIT_EVENTS, P_CGI_PASSES,
+  P_PIECE_MAPPED, P_PIECE_SPLIT_HITS, P_PIECE_SPLIT_EVENTS, P_CGI_PASSES, P_CGI_SPARSE,
   NPATH
 };
 extern const char *const PATH_NAMES[NPATH];

@@ -930,6 +930,77 @@ __global__ void cgi_sum_frag_kernel(unsigned long long *table, uint8_t *touched,
   cgi_sum_pair(table, touched, contigBinOff, genomeContigEnd, totalBins, nGenomes, nQ, oCount, oIdent);
 }
 
+// Sparse stage H: the same reduction from the rows of a piece, with no table over (query, bin) or (query, genome).  Used
+// for pieces whose dense output would dwarf their rows (many small genomes).  Every row gets a key: 1-way winners
+// (query slot << binBits | global bin), the others the sentinel (nQ << binBits), which sorts after every real key.  So a
+// radix sort over the significant bits of all R rows compacts the winners to the front without a host-side count.
+__global__ void cgi_sparse_key_kernel(const CgiArgs a, int binBits, int nQ, unsigned long long *key, uint32_t *row)
+{
+  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= a.R) return;
+  const int f = a.rFrag[i];
+  const int q = a.fragQuery[f];
+  const bani_mapping r = a.rows[i];
+  const int g = a.contigGenome[r.refSeqId];
+  const bool w = cgi_one_way_winner(a, i, f, g, r.nucIdentity);
+  key[i] = w ? ((unsigned long long)q << binBits) | cgi_bin(a, r) : (unsigned long long)nQ << binBits;
+  row[i] = i;
+}
+
+// 1 where a run of equal winner keys -- one (query slot, bin) -- starts; n + 1 flags, the last 0 (exclusive scan -> count)
+__global__ void cgi_sparse_bin_head_kernel(const unsigned long long *key, uint32_t n, unsigned long long sentinel, uint32_t *head)
+{
+  uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j > n) return;
+  head[j] = j < n && key[j] < sentinel && (j == 0 || key[j] != key[j - 1]);
+}
+
+// One thread per bin: its 2-way winner is the row with the largest 64-bit key (identity bits << 32 | querySeqId) -- what
+// the dense path's atomicMax keeps; the pair is unique within a bin, so the winning row is deterministic.  Writes the bin
+// as (query slot << 32 | global bin) with its row, and flags the bins that start a (query slot, genome) pair: bins of a
+// genome are contiguous in the global bin order, so the pairs are runs of the sorted bins.
+__global__ void cgi_sparse_bin_max_kernel(const CgiArgs a, const unsigned long long *key, const uint32_t *row, uint32_t n, int binBits,
+                                          const uint32_t *head, const uint32_t *binIdx,
+                                          unsigned long long *binKey, uint32_t *binRow, uint32_t *pairHead)
+{
+  uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n || !head[j]) return;
+  const unsigned long long k = key[j];
+  uint32_t best = row[j];
+  unsigned long long bestV = cgi_frag_key(a.rows[best]);
+  for (uint32_t t = j + 1; t < n && key[t] == k; t++) {
+    const unsigned long long v = cgi_frag_key(a.rows[row[t]]);
+    if (v > bestV) { bestV = v; best = row[t]; }
+  }
+  const unsigned long long q = k >> binBits, bin = k & ((1ull << binBits) - 1);
+  const uint32_t b = binIdx[j];
+  binKey[b] = (q << 32) | bin;
+  binRow[b] = best;
+  const int g = a.contigGenome[a.rows[best].refSeqId];
+  pairHead[b] = j == 0 || (key[j - 1] >> binBits) != q || a.contigGenome[a.rows[row[j - 1]].refSeqId] != g;
+}
+
+// One thread per (query slot, genome) pair: the float32 sum of its bin winners' identities in ascending bin order, divided
+// by the count -- cgi_sum_pair's order and arithmetic, including its skipping of a bin whose value is 0.  Writes the pair
+// as a bani_cgi_result with the query slot in qryGenomeId (the host maps it), in (query slot, genome) order.
+__global__ void cgi_sparse_pair_kernel(const CgiArgs a, const unsigned long long *binKey, const uint32_t *binRow, const uint32_t *nBinsP,
+                                       const uint32_t *pairHead, const uint32_t *pairIdx, bool fragKeys, bani_cgi_result *out)
+{
+  uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
+  const uint32_t nBins = *nBinsP;
+  if (b >= nBins || !pairHead[b]) return;
+  int32_t cnt = 0; float sum = 0.0f;
+  for (uint32_t t = b; t < nBins && (t == b || !pairHead[t]); t++) {
+    const bani_mapping &r = a.rows[binRow[t]];
+    const unsigned long long v = fragKeys ? cgi_frag_key(r) : (unsigned long long)__float_as_uint(r.nucIdentity);
+    if (v) { sum += r.nucIdentity; cnt++; }
+  }
+  bani_cgi_result o;
+  o.refGenomeId = a.contigGenome[a.rows[binRow[b]].refSeqId]; o.qryGenomeId = (int32_t)(binKey[b] >> 32);
+  o.countSeq = cnt; o.totalQueryFragments = 0; o.identity = cnt ? sum / cnt : 0.0f;
+  out[pairIdx[b]] = o;
+}
+
 // ------------------------------------------------------------------ host orchestration
 __global__ void scount_present_kernel(const int32_t *sCount, int32_t F, int smax, uint32_t *present)
 {
@@ -1069,6 +1140,9 @@ __global__ void compact_sketch_kernel(const uint32_t *raw, const uint32_t *rawSt
 // fragments per piece: the working set of a piece (hit staging, L2 event streams: ~25 GB for 2^18 fragments of config 3)
 // must fit an 80 GB device next to the index of a 1000-genome shard (~32 GB).  The switch frags_per_piece lowers it.
 static constexpr uint64_t FRAG_MAX = 1u << 18;
+// stage H takes the sparse path when a piece's dense (query, genome) output exceeds both its rows and this many entries
+// (32 MB of count + identity): below it the dense tables cost less than the sparse path's sort (DESIGN.md section 6)
+static constexpr uint64_t CGI_SPARSE_MIN_PAIRS = 1u << 22;
 static uint64_t frags_per_piece(const Ctx *ctx) { return std::min<uint64_t>(FRAG_MAX, (uint64_t)std::max(1ll, ctx->flags.fragsPerPiece)); }
 
 // A query as the sketch stage sees it: a contig-length table plus either the packed bases (stage A) or the first contig
@@ -1565,9 +1639,9 @@ void qsketch_map(Ctx *ctx, const Index *ix, const QSketch *const *sketches, int3
     View<int32_t> d_fragQuery; d_fragQuery.p = pc.fragQuery.p; d_fragQuery.n = F;
     View<int32_t> d_fragSeqId; d_fragSeqId.p = pc.fragSeqId.p; d_fragSeqId.n = F;
 
-    std::vector<int32_t> hCount; std::vector<float> hIdent;
+    std::vector<int32_t> hCount; std::vector<float> hIdent;      // dense stage H: allocated once the piece has rows to reduce
+    std::vector<bani_cgi_result> hPairs;                        // sparse stage H: (query slot, genome) rows
     std::vector<bani_frag_mapping> hFrags;
-    if (wantCgi) { hCount.assign((size_t)nQc * nG, 0); hIdent.assign((size_t)nQc * nG, 0.f); }
 
     ctx->mark("piece: begin");
     if (F > 0 && ix->M > 0) {
@@ -1831,8 +1905,66 @@ void qsketch_map(Ctx *ctx, const Index *ix, const QSketch *const *sketches, int3
                 BANI_CUDA(cudaMemcpyAsync(out.rows.data() + old, rows.p, sizeof(bani_mapping) * (size_t)R, cudaMemcpyDeviceToHost, st));
                 BANI_CUDA(cudaStreamSynchronize(st));
               }
-              if (wantCgi) {
+              // ---- H: CGI.  Sparse when the dense (query, genome) output of the piece would exceed both its rows and 2^22
+              // entries (many small genomes; DESIGN.md section 6), unless the cgi_sparse switch forces a path
+              const bool sparse = wantCgi && (ctx->flags.cgiSparse >= 0 ? ctx->flags.cgiSparse == 1
+                                                                        : (uint64_t)nQc * nG > std::max<uint64_t>(R, CGI_SPARSE_MIN_PAIRS));
+              if (sparse) {
+                int qBits = 0; while ((1ull << qBits) <= (uint64_t)nQc) qBits++;                 // slots 0 .. nQc (the sentinel)
+                int binBits = 1; while ((1ull << binBits) < ix->totalBins) binBits++;
+                if (qBits + binBits > 64) fail(BANI_ERR_LIMIT, "sparse identity reduction: %d query bits + %d bin bits exceed 64", qBits, binBits);
+                CgiArgs ca; ca.rows = rows.p; ca.rFrag = rFrag.p; ca.R = R; ca.fragQuery = d_fragQuery.p;
+                ca.contigGenome = ix->contigGenome.p; ca.contigBinOff = ix->contigBinOff.p; ca.fragLen = fragLen;
+                ca.totalBins = ix->totalBins; ca.nGenomes = nG; ca.table = nullptr; ca.touched = nullptr; ca.qLo = 0; ca.qHi = nQc;
+                BANI_SCRATCH(unsigned long long, spKey, R);
+                BANI_SCRATCH(unsigned long long, spKeySorted, R);
+                BANI_SCRATCH(uint32_t, spRow, R);
+                BANI_SCRATCH(uint32_t, spRowSorted, R);
+                BANI_SCRATCH(uint32_t, binHead, (size_t)R + 1);
+                BANI_SCRATCH(uint32_t, binIdx, (size_t)R + 1);
+                BANI_SCRATCH(unsigned long long, binKey, R);
+                BANI_SCRATCH(uint32_t, binRow, R);
+                BANI_SCRATCH(uint32_t, pairHead, (size_t)R + 1);
+                BANI_SCRATCH(uint32_t, pairIdx, (size_t)R + 1);
+                BANI_SCRATCH(bani_cgi_result, dPairs, R);
+                Stage sg(ctx, "cgi_sparse", 150.0 * R);
+                pp[P_CGI_SPARSE]++;
+                cgi_sparse_key_kernel<<<nblk(R), 256, 0, st>>>(ca, binBits, nQc, spKey.p, spRow.p);
+                ctx->launches++;
+                { size_t tb = cub_sort_pairs_u64_u32_temp(R);
+                  BANI_SCRATCH(uint8_t, tmp, tb);
+                  cub_sort_pairs_u64_u32(tmp.p, tb, (const uint64_t *)spKey.p, (uint64_t *)spKeySorted.p, spRow.p, spRowSorted.p, R, qBits + binBits, st); }
+                cgi_sparse_bin_head_kernel<<<nblk((uint64_t)R + 1), 256, 0, st>>>(spKeySorted.p, R, (unsigned long long)nQc << binBits, binHead.p);
+                ctx->launches++;
+                const size_t tbScan = cub_scan_u32_temp((size_t)R + 1);
+                BANI_SCRATCH(uint8_t, scanTmp, tbScan);
+                cub_exclusive_sum_u32(scanTmp.p, tbScan, binHead.p, binIdx.p, (size_t)R + 1, st);
+                BANI_CUDA(cudaMemsetAsync(pairHead.p, 0, 4 * ((size_t)R + 1), st));
+                cgi_sparse_bin_max_kernel<<<nblk(R), 256, 0, st>>>(ca, spKeySorted.p, spRowSorted.p, R, binBits, binHead.p, binIdx.p,
+                                                                   binKey.p, binRow.p, pairHead.p);
+                ctx->launches++;
+                cub_exclusive_sum_u32(scanTmp.p, tbScan, pairHead.p, pairIdx.p, (size_t)R + 1, st);
+                cgi_sparse_pair_kernel<<<nblk(R), 256, 0, st>>>(ca, binKey.p, binRow.p, binIdx.p + R, pairHead.p, pairIdx.p, wantFrags, dPairs.p);
+                ctx->launches++;
+                uint32_t nBins = 0, nPairs = 0;
+                BANI_CUDA(cudaMemcpyAsync(&nBins, binIdx.p + R, 4, cudaMemcpyDeviceToHost, st));
+                BANI_CUDA(cudaMemcpyAsync(&nPairs, pairIdx.p + R, 4, cudaMemcpyDeviceToHost, st));
+                BANI_CUDA(cudaStreamSynchronize(st));
+                // the bin winners are already in (query slot, global bin) order: the fragment rows need no second sort
+                if (wantFrags && nBins > 0) {
+                  BANI_SCRATCH(bani_frag_mapping, dFrags, nBins);
+                  cgi_frag_gather_kernel<<<nblk(nBins), 256, 0, st>>>(rows.p, binKey.p, binRow.p, nBins, dFrags.p);
+                  ctx->launches++;
+                  hFrags.resize(nBins);
+                  BANI_CUDA(cudaMemcpyAsync(hFrags.data(), dFrags.p, sizeof(bani_frag_mapping) * (size_t)nBins, cudaMemcpyDeviceToHost, st));
+                }
+                hPairs.resize(nPairs);
+                if (nPairs) BANI_CUDA(cudaMemcpyAsync(hPairs.data(), dPairs.p, sizeof(bani_cgi_result) * (size_t)nPairs, cudaMemcpyDeviceToHost, st));
+                BANI_CUDA(cudaStreamSynchronize(st));
+                ctx->mark("piece: sparse identity rows on host");
+              } else if (wantCgi) {
                 // ---- H: CGI, at most tableQ queries of the piece per pass over the rows
+                hCount.assign((size_t)nQc * nG, 0); hIdent.assign((size_t)nQc * nG, 0.f);
                 const uint64_t needQ = std::min<uint64_t>(qMaxByTable, std::max<uint64_t>(nQc, 1));
                 if (needQ > tableQ) {
                   tableQ = needQ;
@@ -1916,8 +2048,16 @@ void qsketch_map(Ctx *ctx, const Index *ix, const QSketch *const *sketches, int3
       pp[P_PIECE_MAPPED]++;
       for (int i = 0; i < NPATH; i++) ctx->paths[i] += pp[i];
     }
-    if (wantCgi && !split) {
+    if (wantCgi && !split && !hCount.empty()) {
       append_cgi_rows(hCount.data(), hIdent.data(), nQc, nG, qs->queryId.data() + q0, qs->totalFragments.data() + q0, out.cgi);
+    }
+    if (wantCgi && !split) {
+      for (bani_cgi_result r : hPairs) {
+        if (r.countSeq <= 0) continue;
+        const int slot = r.qryGenomeId;
+        r.qryGenomeId = qs->queryId[q0 + slot]; r.totalQueryFragments = (int32_t)qs->totalFragments[q0 + slot];
+        out.cgi.push_back(r);
+      }
     }
     if (wantFrags && !split) {
       for (auto &m : hFrags) m.qryGenomeId = qs->queryId[q0 + m.qryGenomeId];

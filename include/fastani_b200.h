@@ -134,7 +134,11 @@ BANI_API void *bani_ctx_stream(bani_ctx *ctx);
  * "frags_per_piece" (1 .. 2^18, default 2^18: fragments per query piece; exported sketches do not depend on it),
  * "event_bytes_per_piece" (0 = a quarter of device memory: a piece whose L2 event streams take more is mapped in halves),
  * "cgi_table_queries" (0 = as many as 3 GiB of bin table hold: queries per pass of the identity reduction),
- * "l2_fast" (1; 0 sends every L2 candidate to the exact kernel).  "count_paths" (default 0) turns on the branch counters
+ * "l2_fast" (1; 0 sends every L2 candidate to the exact kernel),
+ * "cgi_sparse" (-1 = chosen per piece: the identity reduction reduces a piece's rows by sorting them when its dense
+ * query x genome output would exceed both the rows and 2^22 entries, as with many small genomes; 0 = always the dense
+ * tables; 1 = always the sorted rows; environment default BANI_CGI_SPARSE, any other value makes bani_ctx_create fail
+ * with BANI_ERR_ARG).  "count_paths" (default 0) turns on the branch counters
  * of bani_ctx_path_counts; with it off the mapping launches exactly the same kernels with the same work.
  * Budgets of a run that builds its reference list in chunks (bani_ctx_plan_run; results never depend on them):
  * "index_bytes_budget" (0 = derived from device memory: the build peak one chunk's index may take) and
@@ -149,7 +153,8 @@ BANI_API int  bani_ctx_set_flag(bani_ctx *ctx, const char *name, int64_t value);
  * lookup.walk_saturated / lookup.walk_full_bucket (probes that walked the sorted keys), l2.events_nt64|128|256,
  * l2.dir1024|4096, l2.staged, l2.direct (L2 candidates with window events, per event-kernel variant), l2.exact_at_bounds /
  * l2.exact_total (candidates left to the exact kernel after the bounds pass / in all), piece.mapped, piece.split_hits,
- * piece.split_events, cgi.passes.  All but piece.split_* describe the pieces that were mapped, not those split. */
+ * piece.split_events, cgi.passes (passes of the dense identity reduction), cgi.sparse (pieces whose identity reduction
+ * took the sparse path).  All but piece.split_* describe the pieces that were mapped, not those split. */
 BANI_API int  bani_ctx_path_counts(bani_ctx *ctx, char (*names)[32], uint64_t *counts, int32_t n_max, int32_t *n);
 
 /* Per-stage device timing.  When enabled, every stage of HP1/HP2 is bracketed by CUDA events on
