@@ -7,6 +7,6 @@ importing works anywhere, but every compute call raises if the library or a GPU 
 from .api import (Parameters, Context, Genome, PackedBatch, Sketch, Map, MapCounters, BaniError,  # noqa: F401
                   MAPPING_DTYPE, MINIMIZER_DTYPE, CGI_DTYPE, FRAG_DTYPE, compute_cgi, compute_cgi_sketched, QuerySketch,
                   load_library, library_path, compute_cgi_chunked, plan_chunks, index_footprint, index_budget,
-                  map_working_set, parse_byte_count, plan_run, run_working_set, index_file_info,
+                  map_working_set, parse_byte_count, plan_run, run_working_set, index_file_info, index_file_extend,
                   compute_cgi_from_index_file)
 from .fasta import read_fasta  # noqa: F401

@@ -128,6 +128,7 @@ def load_library():
         "bani_index_file_info": (C.c_int, [C.c_char_p, P(i32), P(i32), P(i32), P(i32), P(i32), P(u64), P(u64), vp, vp, vp, vp, u64, vp, u64]),
         "bani_index_load_budget": (C.c_int, [vp, C.c_char_p, i32, u64, P(vp), P(i32), P(u64)]),
         "bani_qsketch_from_index_file": (C.c_int, [vp, C.c_char_p, vp, i32, vp, P(vp)]),
+        "bani_index_file_extend": (C.c_int, [vp, C.c_char_p, vp, C.c_char_p]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)          # AttributeError if the ABI lost a symbol
@@ -148,7 +149,7 @@ EXPORTED_SYMBOLS = [
     "bani_qsketch_export", "bani_qsketch_import", "bani_qsketch_merge", "bani_map_cgi_sketch", "bani_map_cgi_sketch_frags",
     "bani_index_build_budget", "bani_ctx_mem_stats", "bani_ctx_trim", "bani_ctx_plan_run", "bani_plan_run", "bani_run_working_set", "bani_index_footprint",
     "bani_map_working_set", "bani_index_budget", "bani_plan_chunks", "bani_qsketch_bytes_estimate", "bani_parse_byte_count",
-    "bani_index_file_info", "bani_index_load_budget", "bani_qsketch_from_index_file"]
+    "bani_index_file_info", "bani_index_load_budget", "bani_qsketch_from_index_file", "bani_index_file_extend"]
 
 
 def _check(rc):
@@ -822,6 +823,15 @@ def index_file_info(path):
     return {"version": ver.value, "k": k.value, "w": w.value, "frag_len": fl.value, "n_genomes": n, "n_contigs": m,
             "n_minimizers": nm.value, "genome_contigs": gc[:n], "genome_length": gl[:n], "genome_records": gr[:n],
             "genome_bits": gb[:n], "contig_length": cl[:m]}
+
+
+def index_file_extend(ctx, in_path, added_sketch, out_path):
+    """bani_index_file_extend: the saved index file in_path (version 3) followed by the genomes of added_sketch (a Sketch on
+    ctx's device), written to out_path byte for byte as Sketch(in_path's genomes + added_sketch's genomes).save(out_path)
+    would write it.  in_path's genomes are not sketched again; its records are streamed through host memory and checked
+    against their checksums.  Raises BaniError (nothing is left at out_path) when out_path is in_path, the parameters
+    differ, in_path is version 2, holds no records or is corrupt, or the joined index exceeds 2^32 minimizers."""
+    _check(ctx.lib.bani_index_file_extend(ctx.h, os.fsencode(in_path), added_sketch.h, os.fsencode(out_path)))
 
 
 def compute_cgi_from_index_file(ctx, path, query_sketches, index_budget=None, query_budget=None):

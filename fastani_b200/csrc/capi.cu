@@ -639,6 +639,16 @@ int bani_index_load_budget(bani_ctx *ctx, const char *path, int32_t first_genome
   BANI_CATCH
 }
 
+int bani_index_file_extend(bani_ctx *ctx, const char *in_path, const bani_index *added, const char *out_path)
+{
+  BANI_TRY
+  if (!ctx || !in_path || !added || !added->ix || !out_path) fail(BANI_ERR_ARG, "null argument");
+  BANI_CUDA(cudaSetDevice(ctx->c.device));
+  index_file_extend(&ctx->c, in_path, added->ix, out_path);
+  return BANI_OK;
+  BANI_CATCH
+}
+
 int bani_index_contigs(const bani_index *ix, int32_t *contig_len, uint64_t cap_contigs, int32_t *seqs_by_file, uint64_t cap_genomes)
 {
   BANI_TRY

@@ -384,6 +384,9 @@ struct IndexFileInfo {
   uint64_t file_bytes() const;
 };
 IndexFileInfo index_file_info(const char *path);
+// The version-3 file inPath followed by the genomes of `added`, written to outPath: equal byte for byte to index_save of the
+// index built from inPath's genomes and then added's.  The old file is streamed through a host buffer and checked on the way.
+void index_file_extend(Ctx *ctx, const char *inPath, const Index *added, const char *outPath);
 // The longest run of genomes [first, first + *nTaken) of a version-3 file whose load (index_footprint of its exact record
 // count, no sketch staging) fits maxBytes, at least one (BANI_ERR_LIMIT if that one does not fit); only that run is read.
 // The index equals index_build's of exactly those genomes.  *peakBytes: most bytes held above the entry.

@@ -16,6 +16,8 @@
 // is outside.
 #include "common.cuh"
 #include <algorithm>
+#include <cstring>
+#include <sys/stat.h>
 
 namespace bani {
 
@@ -551,8 +553,11 @@ struct File {
   FILE *f = nullptr; std::string path; uint64_t sum = 0;
   File(const char *p, const char *mode) : f(fopen(p, mode)), path(p) { if (!f) fail(BANI_ERR_ARG, "cannot open %s", p); }
   ~File() { if (f) fclose(f); }
-  void write(const void *p, size_t n) { if (n && fwrite(p, 1, n, f) != n) fail(BANI_ERR_INTERNAL, "write error on %s", path.c_str()); sum += word_sum(p, n); }
-  void read(void *p, size_t n) { if (n && fread(p, 1, n, f) != n) fail(BANI_ERR_ARG, "%s is truncated", path.c_str()); sum += word_sum(p, n); }
+  void write(const void *p, size_t n) { put(p, n); sum += word_sum(p, n); }
+  void read(void *p, size_t n) { get(p, n); sum += word_sum(p, n); }
+  // the same without adding to `sum`: for callers that sum the words themselves
+  void put(const void *p, size_t n) { if (n && fwrite(p, 1, n, f) != n) fail(BANI_ERR_INTERNAL, "write error on %s", path.c_str()); }
+  void get(void *p, size_t n) { if (n && fread(p, 1, n, f) != n) fail(BANI_ERR_ARG, "%s is truncated", path.c_str()); }
   void seek(uint64_t off) { if (fseeko(f, (off_t)off, SEEK_SET) != 0) fail(BANI_ERR_ARG, "%s: cannot seek to byte %llu", path.c_str(), (unsigned long long)off); }
 };
 
@@ -668,63 +673,121 @@ static void check_file_params(const Ctx *ctx, const IndexFileInfo &x, const char
          path, x.k, x.w, x.fragLen, k, w, fragLen);
 }
 
+namespace {
+// Writes a version-3 file: the header and tables on construction, then the three sections -- hash, wpos, validity bitmap --
+// in order, each given in one or more pieces (device arrays, host words, zeros), then the sums (finish).  Every word of a
+// section is added to the sum of the genome it belongs to on the way (words past the last genome, the trailing bitmap word,
+// count for none) and to the checksum.  A writer destroyed before finish() removes its partial file.  The one place that
+// knows the layout beyond the header: index_save and index_file_extend both write through it.
+class IndexWriter {
+ public:
+  static constexpr size_t CHW = (size_t)16 << 20;          // words per piece of the pinned staging buffer
+  IndexWriter(Ctx *ctx, const char *path, int k, int w, int fragLen, const std::vector<int32_t> &contigLen,
+              const std::vector<int32_t> &seqsByFile, const std::vector<uint32_t> &recOff, uint64_t validWords)
+    : st_(ctx->stream), f_(path, "wb")
+  {
+    try { begin(k, w, fragLen, contigLen, seqsByFile, recOff, validWords); }
+    catch (...) { discard(); throw; }
+  }
+  ~IndexWriter() { if (stage_) cudaFreeHost(stage_); if (!done_) discard(); }
+  IndexWriter(const IndexWriter &) = delete; IndexWriter &operator=(const IndexWriter &) = delete;
+  // the pinned buffer, free between calls: a caller may read host words into it and hand them to host()
+  uint32_t *buffer() { return stage_; }
+  void next_section()
+  {
+    if (sec_ >= 2 || at_ != want_[sec_]) fail(BANI_ERR_INTERNAL, "%s: index section %d written incompletely", f_.path.c_str(), sec_);
+    sec_++; at_ = 0; g_ = 0;
+  }
+  void host(const uint32_t *p, uint64_t n)
+  {
+    f_.put(p, 4 * n);
+    // one pass over the words: each range goes to its genome's sum and to the checksum
+    const std::vector<uint64_t> &ends = sec_ < 2 ? recEnd_ : bitEnd_;
+    for (uint64_t i = 0; i < n;) {
+      while (g_ < ends.size() && ends[g_] <= at_ + i) g_++;
+      const uint64_t e = g_ == ends.size() ? n : std::min<uint64_t>(n, ends[g_] - at_);
+      const uint64_t s = word_sum(p + i, 4 * (e - i));
+      if (g_ < ends.size()) genomeSum_[g_] += s;
+      f_.sum += s;
+      i = e;
+    }
+    at_ += n;
+  }
+  void device(const void *dp, uint64_t n)
+  {
+    for (uint64_t o = 0; o < n; o += CHW) {
+      const uint64_t m = std::min<uint64_t>(CHW, n - o);
+      BANI_CUDA(cudaMemcpyAsync(stage_, (const uint32_t *)dp + o, 4 * m, cudaMemcpyDeviceToHost, st_));
+      BANI_CUDA(cudaStreamSynchronize(st_));
+      host(stage_, m);
+    }
+  }
+  void zeros(uint64_t n)
+  {
+    memset(stage_, 0, 4 * std::min<uint64_t>(CHW, n));
+    for (uint64_t o = 0; o < n; o += CHW) host(stage_, std::min<uint64_t>(CHW, n - o));
+  }
+  const std::vector<uint64_t> &genome_sums() const { return genomeSum_; }
+  void finish()
+  {
+    if (sec_ != 2 || at_ != want_[2]) fail(BANI_ERR_INTERNAL, "%s: index section %d written incompletely", f_.path.c_str(), sec_);
+    f_.write(&tableSum_, 8);
+    f_.write(genomeSum_.data(), 8 * genomeSum_.size());
+    const uint64_t sum = f_.sum;
+    f_.write(&sum, 8);
+    if (fflush(f_.f) != 0) fail(BANI_ERR_INTERNAL, "write error on %s", f_.path.c_str());
+    done_ = true;
+  }
+ private:
+  void begin(int k, int w, int fragLen, const std::vector<int32_t> &contigLen, const std::vector<int32_t> &seqsByFile,
+             const std::vector<uint32_t> &recOff, uint64_t validWords)
+  {
+    const uint64_t nC = contigLen.size(), nG = seqsByFile.size(), M = recOff[nC];
+    const uint64_t h[16] = {IX_MAGIC, 3, (uint64_t)k, (uint64_t)w, (uint64_t)fragLen, M, nC, nG, validWords};
+    f_.write(h, sizeof h);
+    f_.write(contigLen.data(), 4 * nC);
+    f_.write(seqsByFile.data(), 4 * nG);
+    f_.write(recOff.data(), 4 * (nC + 1));
+    tableSum_ = f_.sum;
+    // where every genome's records and bitmap words end (in 32-bit words of the hash / wpos and bitmap sections)
+    recEnd_.resize(nG); bitEnd_.resize(nG);
+    uint64_t bits = 0;
+    for (uint64_t g = 0, c = 0; g < nG; g++) {
+      for (; c < (uint64_t)seqsByFile[g]; c++) bits += ((uint64_t)contigLen[c] + 31) & ~31ull;
+      recEnd_[g] = recOff[seqsByFile[g]];
+      bitEnd_[g] = bits / 32;
+    }
+    want_[0] = want_[1] = M; want_[2] = validWords;
+    genomeSum_.assign(nG, 0);
+    BANI_CUDA(cudaHostAlloc(&stage_, 4 * CHW, cudaHostAllocDefault));
+  }
+  void discard()
+  {
+    if (f_.f) { fclose(f_.f); f_.f = nullptr; }
+    remove(f_.path.c_str());
+  }
+  cudaStream_t st_; File f_;
+  uint32_t *stage_ = nullptr;
+  uint64_t tableSum_ = 0, want_[3] = {0, 0, 0}, at_ = 0;
+  int sec_ = 0; size_t g_ = 0; bool done_ = false;
+  std::vector<uint64_t> recEnd_, bitEnd_, genomeSum_;
+};
+}
+
 void index_save(Ctx *ctx, const Index *ix, const char *path)
 {
   cudaStream_t st = ctx->stream;
   if (ix->device != ctx->device) fail(BANI_ERR_ARG, "index lives on another device");
-  File f(path, "wb");
-  const uint64_t M = ix->M, nC = (uint64_t)ix->nContigs, nG = (uint64_t)ix->nGenomes;
-  const uint64_t validWords = M ? ix->validBits.n : 0;
-  uint64_t h[16] = {IX_MAGIC, 3, (uint64_t)ix->k, (uint64_t)ix->w, (uint64_t)ix->fragLen, M, nC, nG, validWords};
-  f.write(h, sizeof h);
-  f.write(ix->contigLen.data(), 4 * nC);
-  f.write(ix->seqsByFile.data(), 4 * nG);
+  const uint64_t M = ix->M, nC = (uint64_t)ix->nContigs;
   std::vector<uint32_t> recOff(nC + 1);
   BANI_CUDA(cudaMemcpyAsync(recOff.data(), ix->contigRecOff.p, 4 * (nC + 1), cudaMemcpyDeviceToHost, st));
   BANI_CUDA(cudaStreamSynchronize(st));
-  f.write(recOff.data(), 4 * (nC + 1));
-  const uint64_t tableSum = f.sum;
-  // where every genome's records and bitmap words end (in 32-bit words of the hash / wpos and validBits arrays)
-  std::vector<uint64_t> recEnd(nG), bitEnd(nG);
-  {
-    uint64_t bits = 0;
-    for (uint64_t g = 0, c = 0; g < nG; g++) {
-      for (; c < (uint64_t)ix->seqsByFile[g]; c++) bits += ((uint64_t)ix->contigLen[c] + 31) & ~31ull;
-      recEnd[g] = recOff[ix->seqsByFile[g]];
-      bitEnd[g] = bits / 32;
-    }
-  }
-  std::vector<uint64_t> genomeSum(nG, 0);
-  // device arrays through a pinned staging buffer
-  const size_t CHW = (size_t)16 << 20;             // words per piece
-  void *stage = nullptr;
-  BANI_CUDA(cudaHostAlloc(&stage, 4 * CHW, cudaHostAllocDefault));
-  try {
-    auto dump = [&](const void *dp, uint64_t words, const std::vector<uint64_t> &ends) {
-      size_t g = 0;
-      for (uint64_t o = 0; o < words; o += CHW) {
-        const uint64_t n = std::min<uint64_t>(CHW, words - o);
-        BANI_CUDA(cudaMemcpyAsync(stage, (const uint32_t *)dp + o, 4 * n, cudaMemcpyDeviceToHost, st));
-        BANI_CUDA(cudaStreamSynchronize(st));
-        f.write(stage, 4 * n);
-        const uint32_t *w = (const uint32_t *)stage;
-        for (uint64_t i = 0; i < n;) {                  // words past the last genome (the trailing bitmap word) count for none
-          while (g < ends.size() && ends[g] <= o + i) g++;
-          if (g == ends.size()) break;
-          const uint64_t e = std::min<uint64_t>(n, ends[g] - o);
-          genomeSum[g] += word_sum(w + i, 4 * (e - i));
-          i = e;
-        }
-      }
-    };
-    dump(ix->hash.p, M, recEnd); dump(ix->wpos.p, M, recEnd);
-    dump(ix->validBits.p, validWords, bitEnd);
-  } catch (...) { cudaFreeHost(stage); throw; }
-  cudaFreeHost(stage);
-  f.write(&tableSum, 8);
-  f.write(genomeSum.data(), 8 * nG);
-  const uint64_t sum = f.sum;
-  f.write(&sum, 8);
+  const uint64_t validWords = M ? ix->validBits.n : 0;
+  IndexWriter wr(ctx, path, ix->k, ix->w, ix->fragLen, ix->contigLen, ix->seqsByFile, recOff, validWords);
+  wr.device(ix->hash.p, M);
+  wr.next_section(); wr.device(ix->wpos.p, M);
+  wr.next_section(); wr.device(ix->validBits.p, validWords);
+  wr.finish();
 }
 
 // rebuilds the hash-ordered side of an index whose position-ordered side was read from a file
@@ -862,6 +925,79 @@ Index *index_load_budget(Ctx *ctx, const char *path, int32_t first, uint64_t max
     index_finish_loaded(ctx, ix.get());
     return ix.release();
   });
+}
+
+// Records are in (seqId, wpos) order and every contig's bits start on a word, so the index of "old genomes, then added
+// genomes" has each section of the old file followed by the added index's: the tables are joined with the added offsets
+// moved past the old ones, the old records and bitmap words are streamed from the file through the writer's buffer (each
+// genome checked against its sum on the way), the added ones come from the device.  The bitmap of an added index without
+// records is read too: contigs shorter than k + w - 1 have valid positions but no window.  Only an index of contigs that
+// are all shorter than k has no bitmap at all; its words are zero, as the sketch launch of a fresh build leaves them.
+void index_file_extend(Ctx *ctx, const char *inPath, const Index *add, const char *outPath)
+{
+  cudaStream_t st = ctx->stream;
+  if (add->device != ctx->device) fail(BANI_ERR_ARG, "index lives on another device");
+  {
+    struct stat a, b;
+    if (strcmp(inPath, outPath) == 0 || (stat(inPath, &a) == 0 && stat(outPath, &b) == 0 && a.st_dev == b.st_dev && a.st_ino == b.st_ino))
+      fail(BANI_ERR_ARG, "%s is the file being extended: write the extended index to another path", outPath);
+  }
+  File f(inPath, "rb");
+  const IndexFileInfo x = index_file_tables(f);
+  check_file_params(ctx, x, inPath);
+  if (add->k != x.k || add->w != x.w || add->fragLen != x.fragLen)
+    fail(BANI_ERR_ARG, "the added index was built with other parameters (k %d w %d fragLen %d) than %s (k %d w %d fragLen %d)",
+         add->k, add->w, add->fragLen, inPath, x.k, x.w, x.fragLen);
+  if (x.version < 3)
+    fail(BANI_ERR_ARG, "%s was saved in version 2, which has no per-genome checksums: save it again to add genomes to it", inPath);
+  if (x.M == 0)
+    fail(BANI_ERR_ARG, "%s holds no minimizers, so it saved no validity bitmap: build it again with the new genomes", inPath);
+  const uint64_t nC0 = x.nContigs, M0 = x.M, nC1 = (uint64_t)add->nContigs, M1 = add->M;
+  if (M0 + M1 > 0xfffffff0ull)
+    fail(BANI_ERR_LIMIT, "%s (%llu minimizers) and the added genomes (%llu) exceed the 2^32 minimizers of one index file", inPath,
+         (unsigned long long)M0, (unsigned long long)M1);
+  if (nC0 + nC1 > 0x7ffffff0ull) fail(BANI_ERR_LIMIT, "%s and the added genomes exceed the 2^31 contigs of one index file", inPath);
+  // the joined tables
+  std::vector<int32_t> contigLen = x.contigLen, seqsByFile = x.seqsByFile;
+  std::vector<uint32_t> recOff = x.recOff, addRecOff(nC1 + 1);
+  BANI_CUDA(cudaMemcpyAsync(addRecOff.data(), add->contigRecOff.p, 4 * (nC1 + 1), cudaMemcpyDeviceToHost, st));
+  BANI_CUDA(cudaStreamSynchronize(st));
+  uint64_t addBits = 0;
+  for (uint64_t c = 0; c < nC1; c++) {
+    contigLen.push_back(add->contigLen[c]);
+    recOff.push_back((uint32_t)(M0 + addRecOff[c + 1]));
+    addBits += ((uint64_t)add->contigLen[c] + 31) & ~31ull;
+  }
+  for (int32_t e : add->seqsByFile) seqsByFile.push_back((int32_t)(nC0 + e));
+  const uint64_t addWords = addBits / 32;
+  if (add->validBits.n && add->validBits.n < addWords) fail(BANI_ERR_INTERNAL, "added index: validity bitmap shorter than its contigs");
+
+  IndexWriter wr(ctx, outPath, x.k, x.w, x.fragLen, contigLen, seqsByFile, recOff, (x.bitOff[nC0] + addBits) / 32 + 1);
+  auto copy = [&](uint64_t words) {                    // old file -> new file through the writer's buffer
+    for (uint64_t o = 0; o < words; o += IndexWriter::CHW) {
+      const uint64_t n = std::min<uint64_t>(IndexWriter::CHW, words - o);
+      f.get(wr.buffer(), 4 * n);                      // summed once, by the writer: see the checksum below
+      wr.host(wr.buffer(), n);
+    }
+  };
+  copy(M0); wr.device(add->hash.p, M1);
+  wr.next_section(); copy(M0); wr.device(add->wpos.p, M1);
+  wr.next_section(); copy(x.validWords - 1);
+  uint32_t last = 1;
+  f.read(&last, 4);
+  if (last != 0) fail(BANI_ERR_ARG, "%s: corrupt validity bitmap (the word past the last contig is not zero)", inPath);
+  if (add->validBits.n) wr.device(add->validBits.p, addWords); else wr.zeros(addWords);
+  wr.zeros(1);
+  std::vector<uint64_t> want(1 + x.nGenomes);                 // tableSum (checked by index_file_tables), genomeSum[]
+  f.read(want.data(), 8 * want.size());
+  for (uint64_t g = 0; g < x.nGenomes; g++) {
+    if (wr.genome_sums()[g] != want[1 + g]) fail(BANI_ERR_ARG, "%s: checksum mismatch in genome %llu", inPath, (unsigned long long)g);
+    f.sum += want[1 + g];             // every old record and bitmap word but the zero trailing word belongs to a genome
+  }
+  const uint64_t sum = f.sum;
+  uint64_t got = 0;
+  if (fread(&got, 1, 8, f.f) != 8 || got != sum) fail(BANI_ERR_ARG, "%s: checksum mismatch", inPath);
+  wr.finish();
 }
 
 QSketch *qsketch_from_index_file(Ctx *ctx, const char *path, const int32_t *ordinals, int32_t nq, const int32_t *queryIds)

@@ -54,6 +54,10 @@ static void usage(const char *prog, std::ostream &o)
        "     --loadIndex <prefix>  take the references from a saved index instead of -r/--rl: no reference file is read or\n"
        "                           sketched again; queries that are genomes of the index need no file either (one shard).\n"
        "                           Shard files are loaded in chunks that fit the device, on as many GPUs as are visible\n"
+       "     --loadIndex <old> -r/--rl <new genomes> --saveIndex <new>\n"
+       "                           add genomes to a saved index: <new> holds <old>'s genomes, then the new ones, as a fresh\n"
+       "                           --saveIndex of the whole list would (same shards and partition); only the new genomes are\n"
+       "                           read and sketched.  The run then maps the queries against <new>\n"
        "     --visualize           output mappings for visualization (<output>.visual)\n"
        "     --matrix              also output ANI values as lower triangular matrix (<output>.matrix)\n"
        "     -o, --output <value>  output file name\n"
@@ -114,8 +118,13 @@ static void parseandSave(int argc, char **argv, Parameters &p)
   }
   if (help) { usage(argv[0], std::cout); exit(0); }
   if (version) { std::cerr << "version 1.33 (" << bani_version() << ")\n\n"; exit(0); }
-  if (!p.loadIndex.empty() && (!refName.empty() || !refList.empty())) { std::cerr << "ERROR, --loadIndex replaces -r/--rl: give one of them\n"; exit(1); }
-  if (!p.loadIndex.empty() && !p.saveIndex.empty()) { std::cerr << "ERROR, --saveIndex and --loadIndex exclude each other\n"; exit(1); }
+  const bool refsGiven = !refName.empty() || !refList.empty();
+  if (!p.loadIndex.empty() && refsGiven && p.saveIndex.empty()) { std::cerr << "ERROR, --loadIndex replaces -r/--rl: give one of them\n"; exit(1); }
+  if (!p.loadIndex.empty() && !p.saveIndex.empty() && !refsGiven) { std::cerr << "ERROR, --saveIndex and --loadIndex exclude each other\n"; exit(1); }
+  if (!p.loadIndex.empty() && p.saveIndex == p.loadIndex) {
+    std::cerr << "ERROR, --saveIndex " << p.saveIndex << " is the index given to --loadIndex: the index with the added genomes goes to a new prefix\n";
+    exit(1);
+  }
   if (refName.empty() && refList.empty() && p.loadIndex.empty()) { std::cerr << "Provide reference file (s)\n"; exit(1); }
   if (qryName.empty() && qryList.empty()) { std::cerr << "Provide query file (s)\n"; exit(1); }
   if (!refName.empty()) p.refSequences.push_back(refName); else if (!refList.empty()) parseFileList(refList, p.refSequences);
@@ -133,6 +142,10 @@ static void parseandSave(int argc, char **argv, Parameters &p)
   std::cerr << "]\nKmer size = " << p.kmerSize << "\nFragment length = " << p.minReadLength << "\nThreads = " << p.threads
             << "\nANI output file = " << p.outFileName << "\nSanity Check  = " << p.sanityCheck << "\n>>>>>>>>>>>>>>>>>>" << std::endl;
   if (p.loadIndex.empty()) validateInputFiles(p.querySequences, p.refSequences);
+  else for (const auto &e : p.refSequences) {       // genomes added to a loaded index (queries may be genomes of the index)
+    std::ifstream in(e);
+    if (in.fail()) { std::cerr << "ERROR, skch::validateInputFiles, Could not open " << e << std::endl; exit(1); }
+  }
 }
 
 // ---- metadata of a saved index: what the flat per-shard files (bani_index_save) do not hold -- genome paths and
@@ -202,13 +215,20 @@ int main(int argc, char **argv)
   const std::string fileName = parameters.outFileName;
   try {
     const bool loading = !parameters.loadIndex.empty();
+    const bool extending = loading && !parameters.saveIndex.empty();      // -r/--rl genomes added to the loaded index
     IndexMeta meta;
+    std::vector<std::string> addedRefs;
     if (loading) {
       meta = readMeta(parameters.loadIndex);
       if (meta.k != parameters.kmerSize || meta.fragLen != parameters.minReadLength || meta.window != parameters.windowSize)
         throw std::runtime_error("the saved index was built with k " + std::to_string(meta.k) + " fragLen " + std::to_string(meta.fragLen) + " window " + std::to_string(meta.window) +
                                  ", this run asks for k " + std::to_string(parameters.kmerSize) + " fragLen " + std::to_string(parameters.minReadLength) + " window " + std::to_string(parameters.windowSize));
+      if (extending && meta.block && meta.shards > 1)
+        throw std::runtime_error("cannot add genomes to " + parameters.loadIndex + ": its " + std::to_string(meta.shards) + " shards are blocks of the reference "
+                                 "list (--partition block), and a fresh save of the longer list would cut the blocks differently");
+      addedRefs = parameters.refSequences;
       parameters.refSequences = meta.refPaths;
+      parameters.refSequences.insert(parameters.refSequences.end(), addedRefs.begin(), addedRefs.end());
       parameters.blockPartition = meta.block;
     }
     // a run that names its GPU count initialises only those devices (the driver's start-up cost grows with every visible GPU)
@@ -243,7 +263,7 @@ int main(int argc, char **argv)
     auto derivable = [&](const std::string &q) { return deriveQueries && refOrdinal.count(q) > 0; };
     std::unordered_map<std::string, int> pathId; std::vector<std::string> paths;
     for (const auto &e : parameters.querySequences) if (!derivable(e) && !pathId.count(e)) { pathId[e] = (int)paths.size(); paths.push_back(e); }
-    if (!loading) for (const auto &e : parameters.refSequences) if (!pathId.count(e)) { pathId[e] = (int)paths.size(); paths.push_back(e); }
+    for (const auto &e : loading ? addedRefs : parameters.refSequences) if (!pathId.count(e)) { pathId[e] = (int)paths.size(); paths.push_back(e); }
     std::vector<bani_host::HostGenome> genomes(paths.size());
     {
       std::atomic<size_t> next(0); std::mutex emu; std::string err;
@@ -264,6 +284,77 @@ int main(int argc, char **argv)
     std::cerr << "INFO, skch::main, Time spent reading " << paths.size() << " genome files : "
               << std::chrono::duration<double>(Clock::now() - t0).count() << " sec" << std::endl;
     for (int g = 0; g < G; g++) if (!ctxs[g]) throw std::runtime_error("bani_ctx_create: " + ctxErr[g]);
+
+    // ---- genomes added to a saved index: shard file s of the loaded prefix, followed by the added genomes the saved partition
+    //      deals to shard s (list position j goes to shard j mod S), is written to the new prefix by bani_index_file_extend --
+    //      the saved genomes are not sketched again -- and .meta last.  On any failure no file of the new prefix is left.  The
+    //      run then goes on as a --loadIndex run of the new prefix.
+    if (extending) {
+      const int nOld = (int)meta.refPaths.size();
+      std::vector<char> written(S, 0);
+      std::mutex xmu; std::string xerr;
+      auto extendShard = [&](bani_ctx *ctx, int g, int s) {
+        const std::string in = shardFile(parameters.loadIndex, s, S), out = shardFile(parameters.saveIndex, s, S);
+        std::vector<const bani_host::HostGenome *> rh;
+        size_t nSaved = 0;
+        for (int j : shards[s]) { if (j < nOld) nSaved++; else rh.push_back(&genomes[pathId.at(parameters.refSequences[j])]); }
+        const IndexFileTables t = indexFileTables(in);
+        if (t.genomeLen.size() != nSaved)
+          throw std::runtime_error(in + " holds " + std::to_string(t.genomeLen.size()) + " genomes, " + parameters.loadIndex + ".meta gives its shard " + std::to_string(nSaved));
+        std::vector<std::unique_ptr<DeviceGenome>> dev;
+        upload_genomes(ctx, rh, dev, (size_t)1 << 28, std::max(1, parameters.threads / G));
+        std::vector<bani_genome *> hs; for (auto &d : dev) hs.push_back(d->h);
+        const int32_t n = (int32_t)hs.size();
+        auto tooMany = [&](const std::string &why) {
+          return std::runtime_error("the " + std::to_string(n) + " genome(s) added to shard " + std::to_string(s) + " (" + out + ") do not fit one index: " + why +
+                                    ": add fewer genomes per run");
+        };
+        bani_index *ix = nullptr;
+        if (n == 0) check(bani_index_build(ctx, nullptr, 0, &ix), "bani_index_build");
+        else {     // one index at the budget a run plans for these genomes
+          std::vector<uint64_t> rlen; std::vector<int32_t> rcont;
+          for (const auto *h : rh) { uint64_t len = 0; for (const auto &c : h->contigs) len += c.len; rlen.push_back(len); rcont.push_back((int32_t)h->contigs.size()); }
+          std::vector<int32_t> cEnd(n); int32_t nc = 0, nb = 0; uint64_t budget = 0;
+          if (bani_ctx_plan_run(ctx, 0, 0, rlen.data(), rcont.data(), n, nullptr, nullptr, 0, cEnd.data(), &nc, nullptr, &nb, &budget) != BANI_OK)
+            throw tooMany(bani_last_error());
+          int32_t taken = n;
+          const int rc = budget ? bani_index_build_budget(ctx, hs.data(), n, budget, &ix, &taken, nullptr) : bani_index_build(ctx, hs.data(), n, &ix);
+          if (rc == BANI_ERR_LIMIT) throw tooMany(bani_last_error());
+          check(rc, "bani_index_build_budget");
+          if (taken < n) {
+            bani_index_destroy(ix);
+            throw tooMany("the index budget of " + std::to_string(budget) + " bytes holds the first " + std::to_string(taken));
+          }
+        }
+        std::unique_ptr<bani_index, void (*)(bani_index *)> ixOwner(ix, bani_index_destroy);
+        uint64_t added = 0;
+        check(bani_index_stats(ix, &added, nullptr, nullptr, nullptr, nullptr), "bani_index_stats");
+        check(bani_index_file_extend(ctx, in.c_str(), ix, out.c_str()), "bani_index_file_extend");
+        written[s] = 1;
+        ixOwner.reset(); dev.clear();
+        check(bani_ctx_trim(ctx), "bani_ctx_trim");
+        for (const auto *h : rh) for (const auto &c : h->contigs) meta.contigNames[s].push_back(c.name);
+        std::lock_guard<std::mutex> l(xmu);
+        std::cerr << "INFO [GPU " << g << "], skch::main, shard file " << s << ": " << n << " genome(s) and " << added << " minimizers added to "
+                  << in << " -> " << out << std::endl;
+      };
+      {
+        std::vector<std::thread> th;
+        for (int g = 0; g < G; g++)
+          th.emplace_back([&, g]() {
+            try { for (int s = g; s < S; s += G) extendShard(ctxs[g], g, s); }
+            catch (const std::exception &e) { std::lock_guard<std::mutex> l(xmu); xerr = e.what(); }
+          });
+        for (auto &t : th) t.join();
+      }
+      auto removeWritten = [&]() { for (int s = 0; s < S; s++) if (written[s]) std::remove(shardFile(parameters.saveIndex, s, S).c_str()); };
+      if (!xerr.empty()) { removeWritten(); throw std::runtime_error(xerr); }
+      try { writeMeta(parameters.saveIndex, parameters, S, meta.contigNames); }
+      catch (...) { removeWritten(); std::remove((parameters.saveIndex + ".meta").c_str()); throw; }
+      meta.refPaths = parameters.refSequences;
+      parameters.loadIndex = parameters.saveIndex;
+      parameters.saveIndex.clear();
+    }
 
     std::vector<cgi::CGI_Results> finalResults;
     std::vector<std::string> visual(S);

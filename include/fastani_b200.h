@@ -323,6 +323,15 @@ BANI_API int  bani_index_file_info(const char *path, int32_t *version, int32_t *
  * call held above what was held on entry.  Same k / window / fragLen as the context, as for bani_index_load. */
 BANI_API int  bani_index_load_budget(bani_ctx *ctx, const char *path, int32_t first_genome, uint64_t max_bytes, bani_index **out,
                                      int32_t *n_taken, uint64_t *peak_bytes);
+/* The saved index file in_path (version 3) followed by the genomes of `added` (an index on ctx's device), written to
+ * out_path: equal byte for byte to bani_index_save of bani_index_build(in_path's genomes, then added's genomes).  The
+ * saved genomes are not sketched again: in_path is streamed through a fixed host buffer, never loaded onto the device,
+ * and each of its genomes is checked against its checksum on the way (a mismatch names the genome).  added may hold no
+ * records (genomes whose contigs are all shorter than k + w - 1).  BANI_ERR_ARG: out_path is in_path, in_path has other
+ * k / window / fragLen than the context, is version 2 (save it again), holds no records (build it again with the new
+ * genomes) or is corrupt.  BANI_ERR_LIMIT: the joined index exceeds 2^32 minimizers.  On any failure no file is left at
+ * out_path. */
+BANI_API int  bani_index_file_extend(bani_ctx *ctx, const char *in_path, const bani_index *added, const char *out_path);
 
 /* ---- HP2: query mapping ---------------------------------------------------
  * Map::mapQuery (computeMap.hpp:112-196) for one query genome: every mapping the
