@@ -402,6 +402,15 @@ inline std::vector<std::vector<int>> splitReferenceGenomes(int nRefs, int G, boo
   else for (int j = 0; j < nRefs; j++) s[j % G].push_back(j);
   return s;
 }
+// the inverse of splitReferenceGenomes: list position j -> (shard, ordinal inside the shard)
+inline std::pair<int, int> referenceShardOrdinal(int j, int nRefs, int G, bool block = false)
+{
+  if (!block) return {j % G, j / G};
+  auto start = [&](int g) { return (int)((int64_t)nRefs * g / G); };
+  int g = (int)((int64_t)j * G / nRefs);                  // start(g) <= j; shards before j's may be empty (nRefs < G)
+  while (g + 1 < G && start(g + 1) <= j) g++;
+  return {g, j - start(g)};
+}
 // computeCoreIdentity.hpp:480-487: shard-local reference id -> global id
 inline void correctRefGenomeIds(std::vector<CGI_Results> &v, int shard, int G, int nRefs = 0, bool block = false)
 {

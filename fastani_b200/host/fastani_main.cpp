@@ -13,7 +13,9 @@
 //   * the per-pair reduction runs on the device for every query of a GPU at once (bani_map_cgi_sketch); with --visualize
 //     it also returns the 2-way fragment mappings the .visual file is written from (bani_map_cgi_sketch_frags).
 //     BANI_CLI_HOST_CGI=1 (a test switch) instead maps one query at a time, copies its mapping rows back and runs
-//     cgi::computeCGI on the host, so that both paths can be compared on the same inputs
+//     cgi::computeCGI on the host, so that both paths can be compared on the same inputs.  The same switch makes a
+//     --loadIndex run read and hash every query file, also those of genomes of the index (whose sketches are otherwise
+//     derived from the shard file that holds them)
 #include <atomic>
 #include <chrono>
 #include <cstdlib>
@@ -52,7 +54,7 @@ static void usage(const char *prog, std::ostream &o)
        "                           deal, default) or block (contiguous ranges: list neighbours stay on one GPU)\n"
        "     --saveIndex <prefix>  write the reference sketches to <prefix>.meta + <prefix>.<shard>of<N>.idx after building them\n"
        "     --loadIndex <prefix>  take the references from a saved index instead of -r/--rl: no reference file is read or\n"
-       "                           sketched again; queries that are genomes of the index need no file either (one shard).\n"
+       "                           sketched again; queries that are genomes of the index need no file either.\n"
        "                           Shard files are loaded in chunks that fit the device, on as many GPUs as are visible\n"
        "     --loadIndex <old> -r/--rl <new genomes> --saveIndex <new>\n"
        "                           add genomes to a saved index: <new> holds <old>'s genomes, then the new ones, as a fresh\n"
@@ -252,17 +254,28 @@ int main(int argc, char **argv)
     for (int g = 0; g < G; g++)
       ctxThreads.emplace_back([&, g]() { bani_params cp = parameters.c(); if (bani_ctx_create(g, &cp, &ctxs[g]) != BANI_OK) ctxErr[g] = bani_last_error(); });
 
-    // ---- ingest: every distinct file once, in parallel.  With a loaded index no reference file is read, and (one
-    //      shard) neither is a query that is a genome of the index: its sketch is derived from the index
+    // ---- ingest: every distinct file once, in parallel.  With a loaded index no reference file is read, and neither is
+    //      a member query -- one whose path is a genome of the index (its first position in the list): its sketch is derived
+    //      from the shard file that holds the genome
     auto t0 = Clock::now();
     std::unordered_map<std::string, int> refOrdinal;                  // path -> first position in the reference list
     for (size_t j = 0; j < parameters.refSequences.size(); j++) refOrdinal.emplace(parameters.refSequences[j], (int)j);
     const char *hostCgiEnv = getenv("BANI_CLI_HOST_CGI");
-    const bool hostCgi = parameters.visualize && hostCgiEnv && atoi(hostCgiEnv) != 0;     // per-query host computeCGI (test switch)
-    const bool deriveQueries = loading && meta.shards == 1 && !hostCgi;
-    auto derivable = [&](const std::string &q) { return deriveQueries && refOrdinal.count(q) > 0; };
+    const bool hostCgiSwitch = hostCgiEnv && atoi(hostCgiEnv) != 0;
+    const bool hostCgi = parameters.visualize && hostCgiSwitch;         // per-query host computeCGI (test switch)
+    const bool deriveQueries = loading && !hostCgiSwitch;
+    std::vector<std::pair<int, int>> memberAt(parameters.querySequences.size(), {-1, -1});     // (shard file, ordinal) of a member query
+    if (deriveQueries)
+      for (size_t q = 0; q < memberAt.size(); q++) {
+        const auto it = refOrdinal.find(parameters.querySequences[q]);
+        if (it != refOrdinal.end()) memberAt[q] = cgi::referenceShardOrdinal(it->second, (int)parameters.refSequences.size(), S, parameters.blockPartition);
+      }
+    auto derivable = [&](size_t q) { return memberAt[q].first >= 0; };
     std::unordered_map<std::string, int> pathId; std::vector<std::string> paths;
-    for (const auto &e : parameters.querySequences) if (!derivable(e) && !pathId.count(e)) { pathId[e] = (int)paths.size(); paths.push_back(e); }
+    for (size_t q = 0; q < parameters.querySequences.size(); q++) {
+      const std::string &e = parameters.querySequences[q];
+      if (!derivable(q) && !pathId.count(e)) { pathId[e] = (int)paths.size(); paths.push_back(e); }
+    }
     for (const auto &e : loading ? addedRefs : parameters.refSequences) if (!pathId.count(e)) { pathId[e] = (int)paths.size(); paths.push_back(e); }
     std::vector<bani_host::HostGenome> genomes(paths.size());
     {
@@ -356,6 +369,23 @@ int main(int argc, char **argv)
       parameters.saveIndex.clear();
     }
 
+    // ---- a loaded index: the tables of every shard file, read once -- the genome sizes of the run plans (a member query's
+    //      from the file that holds it), the --minFraction lengths and the contig lengths of the member queries' .visual lines
+    std::vector<IndexFileTables> fileTables;
+    if (loading)
+      for (int s = 0; s < S; s++) {
+        const std::string file = shardFile(parameters.loadIndex, s, S);
+        fileTables.push_back(indexFileTables(file));
+        const IndexFileTables &t = fileTables.back();
+        if (t.genomeLen.size() != shards[s].size())
+          throw std::runtime_error(file + " holds " + std::to_string(t.genomeLen.size()) + " genomes, " + parameters.loadIndex + ".meta gives its shard " +
+                                   std::to_string(shards[s].size()));
+        for (size_t i = 0; i < shards[s].size(); i++) {
+          const int c0 = i ? t.seqsByFile[i - 1] : 0;
+          genomeLengths.emplace(parameters.refSequences[shards[s][i]], cgi::genomeLength(t.contigLen, c0, t.seqsByFile[i], parameters.minReadLength));
+        }
+      }
+
     std::vector<cgi::CGI_Results> finalResults;
     std::vector<std::string> visual(S);
     std::vector<char> sanity(S, 1); std::vector<float> ratioDiffs(S, 1.0f);
@@ -384,31 +414,55 @@ int main(int argc, char **argv)
       bani_free(res);
     };
 
-    // The sketches of query block [q0, q1): queries read from their files are hashed (their device genomes are freed
-    // again); with derive (a loaded one-shard index) the genomes of the index come from its file instead
-    auto blockSketches = [&](bani_ctx *ctx, int q0, int q1, int threads, const std::string &derivedFrom) {
-      std::vector<const bani_host::HostGenome *> qh; std::vector<int32_t> qid, dord, did;
-      for (int q = q0; q < q1; q++) {
-        const std::string &path = parameters.querySequences[q];
-        if (!derivedFrom.empty() && derivable(path)) { dord.push_back(refOrdinal.at(path)); did.push_back(q); }
-        else { qh.push_back(&genomes[pathId.at(path)]); qid.push_back(q); }
-      }
-      std::vector<bani_qsketch *> sk;
+    // The sketch of the queries of block [q0, q1) that are read from their files (null if there are none): they are hashed
+    // and their device genomes freed again
+    auto hashedSketch = [&](bani_ctx *ctx, int q0, int q1, int threads) {
+      std::vector<const bani_host::HostGenome *> qh; std::vector<int32_t> qid;
+      for (int q = q0; q < q1; q++)
+        if (!derivable(q)) { qh.push_back(&genomes[pathId.at(parameters.querySequences[q])]); qid.push_back(q); }
+      bani_qsketch *qsk = nullptr;
       if (!qh.empty()) {
         std::vector<std::unique_ptr<DeviceGenome>> dq;
         upload_genomes(ctx, qh, dq, (size_t)1 << 28, threads);
         std::vector<bani_genome *> hs; for (auto &d : dq) hs.push_back(d->h);
-        bani_qsketch *qsk = nullptr;
         check(bani_qsketch_create(ctx, hs.data(), (int32_t)hs.size(), qid.data(), nullptr, &qsk), "bani_qsketch_create");
-        sk.push_back(qsk);
       }
-      if (!dord.empty()) {
-        bani_qsketch *qsk = nullptr;
-        const int rc = bani_qsketch_from_index_file(ctx, derivedFrom.c_str(), dord.data(), (int32_t)dord.size(), did.data(), &qsk);
-        if (rc != BANI_OK) { for (auto *x : sk) bani_qsketch_destroy(x); check(rc, "bani_qsketch_from_index_file"); }
-        sk.push_back(qsk);
+      return qsk;
+    };
+
+    // The sketches of the member queries of block [q0, q1), derived from the shard files that hold them: one
+    // bani_qsketch_from_index_file call per file, which reads only those genomes and checks each against its checksum.  A
+    // GPU keeps the sketches of its most recent block range, so that the shard files it maps in turn with the same query
+    // blocks derive them once.
+    struct MemberSketches {
+      int q0 = -1, q1 = -1;
+      std::vector<bani_qsketch *> sk;
+      void clear() { for (auto *x : sk) bani_qsketch_destroy(x); sk.clear(); q0 = q1 = -1; }
+    };
+    std::vector<MemberSketches> memberCache(G);
+    auto memberSketches = [&](bani_ctx *ctx, int g, int q0, int q1) -> const std::vector<bani_qsketch *> & {
+      MemberSketches &c = memberCache[g];
+      if (c.q0 == q0 && c.q1 == q1) return c.sk;
+      c.clear();
+      std::vector<std::vector<int32_t>> ord(S), qid(S);
+      for (int q = q0; q < q1; q++)
+        if (derivable(q)) { ord[memberAt[q].first].push_back(memberAt[q].second); qid[memberAt[q].first].push_back(q); }
+      for (int f = 0; f < S; f++) {
+        if (ord[f].empty()) continue;
+        const std::string file = shardFile(parameters.loadIndex, f, S);
+        bani_qsketch *x = nullptr;
+        if (bani_qsketch_from_index_file(ctx, file.c_str(), ord[f].data(), (int32_t)ord[f].size(), qid[f].data(), &x) == BANI_OK) { c.sk.push_back(x); continue; }
+        std::string why = bani_last_error(), who = "one of " + std::to_string(ord[f].size()) + " query genomes";
+        for (size_t i = 0; i < ord[f].size(); i++) {           // name the member whose records fail
+          bani_qsketch *y = nullptr;
+          if (bani_qsketch_from_index_file(ctx, file.c_str(), &ord[f][i], 1, &qid[f][i], &y) == BANI_OK) { bani_qsketch_destroy(y); continue; }
+          why = bani_last_error(); who = "query genome " + parameters.querySequences[qid[f][i]];
+          break;
+        }
+        throw std::runtime_error("cannot derive the sketch of " + who + " from " + file + ": " + why);
       }
-      return sk;
+      c.q0 = q0; c.q1 = q1;
+      return c.sk;
     };
 
     // A shard whose index does not fit the device at once.  Per query block: the block's sketches are made; then the shard's
@@ -416,15 +470,16 @@ int main(int argc, char **argv)
     // budget: genomes it did not take stay uploaded for the next chunk) or loaded from the shard's saved file (the longest
     // run from `first` that fits) -- each mapped, and the index and the cached blocks handed back before the next chunk.
     // Results carry shard-local reference ordinals, as those of one index would.
-    auto chunkedShard = [&](bani_ctx *ctx, int s, const std::vector<int> &shard, const std::vector<std::pair<int, int>> &chunks,
+    auto chunkedShard = [&](bani_ctx *ctx, int g, int s, const std::vector<int> &shard, const std::vector<std::pair<int, int>> &chunks,
                             const std::vector<std::pair<int, int>> &blocks, uint64_t indexBudget, std::vector<cgi::CGI_Results> &local) {
       const int threads = std::max(1, parameters.threads / G);
       const std::string file = loading ? shardFile(parameters.loadIndex, s, S) : std::string();
       int chunkNo = 0;
       for (size_t b = 0; b < blocks.size(); b++) {
-        std::vector<bani_qsketch *> sk = blockSketches(ctx, blocks[b].first, blocks[b].second, threads, deriveQueries ? file : std::string());
-        std::vector<std::unique_ptr<bani_qsketch, void (*)(bani_qsketch *)>> skOwner;
-        for (auto *x : sk) skOwner.emplace_back(x, bani_qsketch_destroy);
+        std::unique_ptr<bani_qsketch, void (*)(bani_qsketch *)> hashed(hashedSketch(ctx, blocks[b].first, blocks[b].second, threads), bani_qsketch_destroy);
+        std::vector<bani_qsketch *> sk;
+        if (hashed) sk.push_back(hashed.get());
+        if (deriveQueries) { const auto &m = memberSketches(ctx, g, blocks[b].first, blocks[b].second); sk.insert(sk.end(), m.begin(), m.end()); }
         std::vector<std::unique_ptr<DeviceGenome>> pending;
         int first = 0;
         size_t next = 0;
@@ -461,18 +516,8 @@ int main(int argc, char **argv)
       uint64_t indexBudget = 0;
       const auto &qs = parameters.querySequences;
       std::vector<uint64_t> qlen(qs.size()), rlen; std::vector<int32_t> rcont;
-      if (loading) {                     // the saved shard file's tables: genome sizes for the plan and the --minFraction filter
-        const IndexFileTables t = indexFileTables(shardFile(parameters.loadIndex, s, S));
-        if (t.genomeLen.size() != shards[s].size())
-          throw std::runtime_error(shardFile(parameters.loadIndex, s, S) + " holds " + std::to_string(t.genomeLen.size()) + " genomes, " +
-                                   parameters.loadIndex + ".meta gives its shard " + std::to_string(shards[s].size()));
-        rlen = t.genomeLen; rcont = t.genomeContigs;
-        std::lock_guard<std::mutex> l(mu);
-        for (size_t i = 0; i < shards[s].size(); i++) {
-          const int c0 = i ? t.seqsByFile[i - 1] : 0;
-          genomeLengths.emplace(parameters.refSequences[shards[s][i]], cgi::genomeLength(t.contigLen, c0, t.seqsByFile[i], parameters.minReadLength));
-        }
-      } else {
+      if (loading) { rlen = fileTables[s].genomeLen; rcont = fileTables[s].genomeContigs; }     // the saved shard file's genome sizes
+      else {
         for (int j : shards[s]) {
           const auto &h = genomes[pathId.at(parameters.refSequences[j])];
           uint64_t len = 0; for (const auto &c : h.contigs) len += c.len;
@@ -480,7 +525,7 @@ int main(int argc, char **argv)
         }
       }
       for (size_t q = 0; q < qs.size(); q++) {
-        if (derivable(qs[q])) { qlen[q] = rlen[refOrdinal.at(qs[q])]; continue; }      // one shard: its ordinal in the file
+        if (derivable(q)) { qlen[q] = fileTables[memberAt[q].first].genomeLen[memberAt[q].second]; continue; }     // from the file that holds it
         for (const auto &c : genomes[pathId.at(qs[q])].contigs) qlen[q] += c.len;
       }
       std::vector<int32_t> cEnd(std::max<size_t>(rlen.size(), 1)), bEnd(std::max<size_t>(qs.size(), 1));
@@ -494,6 +539,8 @@ int main(int argc, char **argv)
         std::cerr << "INFO [GPU " << g << "], skch::main, " << (loading ? "shard file " + std::to_string(s) + ", " : std::string())
                   << "reference chunks : " << chunks.size() << ", query blocks : " << blocks.size() << " (index budget " << indexBudget << " bytes)" << std::endl;
       }
+      // member sketches of another block range than this shard's first block would only take device memory from its index
+      if (memberCache[g].q0 != blocks[0].first || memberCache[g].q1 != blocks[0].second) memberCache[g].clear();
       if (chunks.size() > 1 || blocks.size() > 1) {
         if (parameters.visualize)
           throw std::runtime_error("--visualize needs the reference shard of a GPU in one index, this run needs " + std::to_string(chunks.size()) +
@@ -502,7 +549,7 @@ int main(int argc, char **argv)
           throw std::runtime_error("--saveIndex writes one index per GPU, this run needs " + std::to_string(chunks.size()) + " chunk(s) and " +
                                    std::to_string(blocks.size()) + " query block(s) on GPU " + std::to_string(g) + ": use more GPUs or fewer references");
         std::vector<cgi::CGI_Results> local;
-        chunkedShard(ctx, s, shards[s], chunks, blocks, indexBudget, local);
+        chunkedShard(ctx, g, s, shards[s], chunks, blocks, indexBudget, local);
         if (g == 0) std::cerr << "INFO [GPU 0], skch::main, Time spent " << (loading ? "loading" : "sketching") << " and mapping in chunks : "
                               << std::chrono::duration<double>(Clock::now() - t1).count() << " sec" << std::endl;
         cgi::correctRefGenomeIds(local, s, S, (int)parameters.refSequences.size(), parameters.blockPartition);
@@ -515,7 +562,7 @@ int main(int argc, char **argv)
       auto want = [&](const std::string &path) { const int id = pathId.at(path); if (!slot.count(id)) { slot[id] = (int)need.size(); need.push_back(id); } return slot[id]; };
       std::vector<int> refSlot, qrySlot;                              // qrySlot: -1 = derived from the index
       if (!loading) for (int j : shards[s]) refSlot.push_back(want(parameters.refSequences[j]));
-      for (const auto &q : parameters.querySequences) qrySlot.push_back(derivable(q) ? -1 : want(q));
+      for (size_t q = 0; q < qs.size(); q++) qrySlot.push_back(derivable(q) ? -1 : want(qs[q]));
       std::vector<const bani_host::HostGenome *> hs; for (int id : need) hs.push_back(&genomes[id]);
       std::vector<std::unique_ptr<DeviceGenome>> dev;
       upload_genomes(ctx, hs, dev, (size_t)1 << 28, std::max(1, parameters.threads / G));
@@ -551,21 +598,25 @@ int main(int argc, char **argv)
           }
           visual[s] = vis.str();
         } else {
-          // HP2 + reduction for all queries: one sketch object for the queries that were read, one for those derived
+          // HP2 + reduction for all queries: one sketch object for the queries that were read, and those derived -- from
+          // the loaded index itself when it is the only shard, else one per shard file that holds members (kept for the
+          // GPU's next shard file)
           std::vector<bani_genome *> qh; std::vector<int32_t> qid, dord, did;
           for (size_t q = 0; q < qrySlot.size(); q++) {
             if (qrySlot[q] >= 0) { qh.push_back(dev[qrySlot[q]]->h); qid.push_back((int32_t)q); }
-            else { dord.push_back(refOrdinal.at(parameters.querySequences[q])); did.push_back((int32_t)q); }
+            else { dord.push_back(memberAt[q].second); did.push_back((int32_t)q); }
           }
           std::vector<bani_qsketch *> sk;
           if (!qh.empty()) { bani_qsketch *x = nullptr; check(bani_qsketch_create(ctx, qh.data(), (int32_t)qh.size(), qid.data(), referSketch.handle(), &x), "bani_qsketch_create"); sk.push_back(x); }
-          if (!dord.empty()) { bani_qsketch *x = nullptr; check(bani_qsketch_from_index(ctx, referSketch.handle(), dord.data(), (int32_t)dord.size(), did.data(), &x), "bani_qsketch_from_index"); sk.push_back(x); }
+          if (!dord.empty() && S == 1) { bani_qsketch *x = nullptr; check(bani_qsketch_from_index(ctx, referSketch.handle(), dord.data(), (int32_t)dord.size(), did.data(), &x), "bani_qsketch_from_index"); sk.push_back(x); }
+          const size_t owned = sk.size();
+          if (!dord.empty() && S > 1) { const auto &m = memberSketches(ctx, g, 0, (int)qs.size()); sk.insert(sk.end(), m.begin(), m.end()); }
           bani_cgi_result *res = nullptr; uint64_t n = 0; bani_map_counters ctr;
           bani_frag_mapping *frags = nullptr; uint64_t nf = 0;
           const int rc = parameters.visualize                                                                  // HP2 + reduction
             ? bani_map_cgi_sketch_frags(ctx, referSketch.handle(), sk.data(), (int32_t)sk.size(), &res, &n, &frags, &nf, &ctr)
             : bani_map_cgi_sketch(ctx, referSketch.handle(), sk.data(), (int32_t)sk.size(), &res, &n, &ctr);
-          for (auto *x : sk) bani_qsketch_destroy(x);
+          for (size_t i = 0; i < owned; i++) bani_qsketch_destroy(sk[i]);
           check(rc, parameters.visualize ? "bani_map_cgi_sketch_frags" : "bani_map_cgi_sketch");
           for (uint64_t i = 0; i < n; i++)
             local.push_back(cgi::CGI_Results{res[i].refGenomeId, res[i].qryGenomeId, res[i].countSeq, res[i].totalQueryFragments, res[i].identity});
@@ -582,14 +633,14 @@ int main(int argc, char **argv)
               const int32_t q = frags[i].qryGenomeId;
               uint64_t j = i;
               while (j < nf && frags[j].qryGenomeId == q) j++;
-              // Map::metadata of the query: from its file, or (derived query) from its contigs in the index
+              // Map::metadata of the query: from its file, or (derived query) from its contigs in the shard file that holds it
               std::vector<skch::offset_t> qLens;
               if (qrySlot[q] >= 0) {
                 for (const auto &c : dev[qrySlot[q]]->host->contigs) appendFragmentLengths(parameters, (offset_t)c.len, qLens);
               } else {
-                const int o = refOrdinal.at(parameters.querySequences[q]);
-                const int c0 = o ? referSketch.sequencesByFileInfo[o - 1] : 0, c1 = referSketch.sequencesByFileInfo[o];
-                for (int c = c0; c < c1; c++) appendFragmentLengths(parameters, referSketch.metadata[c].len, qLens);
+                const IndexFileTables &t = fileTables[memberAt[q].first];
+                const int o = memberAt[q].second, c0 = o ? t.seqsByFile[o - 1] : 0, c1 = t.seqsByFile[o];
+                for (int c = c0; c < c1; c++) appendFragmentLengths(parameters, t.contigLen[c], qLens);
               }
               cgi::outputVisualizationFile(parameters, frags + i, j - i, cgi::offsetAdder(qLens), refOff, referSketch,
                                            parameters.querySequences[q], shardRefNames, vis);
@@ -610,8 +661,9 @@ int main(int argc, char **argv)
     auto gpuWork = [&](int g) {
       try {
         for (int s = g; s < S; s += G) shardRun(ctxs[g], g, s);
+        memberCache[g].clear();
         if (getenv("BANI_CLI_FULL_TEARDOWN")) bani_ctx_destroy(ctxs[g]);      // otherwise the process exit returns the device memory (faster)
-      } catch (const std::exception &e) { std::lock_guard<std::mutex> l(mu); err = e.what(); }
+      } catch (const std::exception &e) { memberCache[g].clear(); std::lock_guard<std::mutex> l(mu); err = e.what(); }
     };
     {
       std::vector<std::thread> th;
