@@ -9,7 +9,7 @@ CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "lib")
 LIB = os.path.join(OUT, "libfastani_b200.so")
 STAMP = os.path.join(OUT, "flags.txt")
-SOURCES = ["capi.cu", "pack.cu", "sketch.cu", "index.cu", "map.cu", "hits.cu", "synth.cu", "cubops.cu", "stats.cpp", "alloc.cpp", "budget.cpp"]
+SOURCES = ["capi.cu", "pack.cu", "sketch.cu", "index.cu", "map.cu", "cgi.cu", "hits.cu", "synth.cu", "cubops.cu", "stats.cpp", "alloc.cpp", "budget.cpp"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = GENCODE + ["-O3", "-lineinfo", "-std=c++17",

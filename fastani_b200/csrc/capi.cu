@@ -155,7 +155,7 @@ void bani_ctx_destroy(bani_ctx *ctx)
   cudaSetDevice(ctx->c.device);
   cudaStreamSynchronize(ctx->c.stream);
   ctx->c.d_minHits.release(); ctx->c.d_rowOff.release(); ctx->c.d_ident.release(); ctx->c.d_upper.release();
-  ctx->c.slots.clear();
+  ctx->c.slots.clear(); ctx->c.cubTemp.release();
   cudaStreamSynchronize(ctx->c.stream);
   cudaStreamSynchronize(ctx->c.copyStream);
   dev_cache_flush(ctx->c.device);            // blocks are keyed by stream: return them before it dies
@@ -285,7 +285,7 @@ int bani_ctx_trim(bani_ctx *ctx)
   if (!ctx) fail(BANI_ERR_ARG, "null context");
   BANI_CUDA(cudaSetDevice(ctx->c.device));
   BANI_CUDA(cudaStreamSynchronize(ctx->c.stream));
-  ctx->c.slots.clear();
+  ctx->c.slots.clear(); ctx->c.cubTemp.release();
   dev_cache_flush(ctx->c.device);
   return BANI_OK;
   BANI_CATCH

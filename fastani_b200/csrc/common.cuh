@@ -10,6 +10,7 @@
 #include <cstdio>
 #include <cstdarg>
 #include <chrono>
+#include <type_traits>
 #include "../../include/fastani_b200.h"
 
 namespace bani {
@@ -191,12 +192,10 @@ struct Index {
   uint64_t totalBins = 0;
 };
 
-// A non-owning typed view of a persistent scratch slot (same surface as DevBuf where it is used).
+// A non-owning typed view of a persistent scratch slot.
 template <typename T>
 struct View {
   T *p = nullptr; size_t n = 0;
-  size_t bytes() const { return n * sizeof(T); }
-  void release() {}
 };
 
 // Run-time switches of a context (bani_ctx_set_flag); the defaults can also be set through the environment
@@ -240,6 +239,21 @@ enum PathId {
 };
 extern const char *const PATH_NAMES[NPATH];
 
+// CUB-backed primitives (cubops.cu; kept in one TU because CUB compiles slowly)
+size_t cub_sort_pairs_u32_temp(size_t n);
+void   cub_sort_pairs_u32(void *temp, size_t tempBytes, const uint32_t *kin, uint32_t *kout,
+                          const uint32_t *vin, uint32_t *vout, size_t n, int endBit, cudaStream_t s);
+size_t cub_sort_keys_u64_temp(size_t n);
+void   cub_sort_keys_u64(void *temp, size_t tempBytes, const uint64_t *kin, uint64_t *kout, size_t n,
+                         int beginBit, int endBit, cudaStream_t s);
+size_t cub_sort_pairs_u64_u32_temp(size_t n);
+void   cub_sort_pairs_u64_u32(void *temp, size_t tempBytes, const uint64_t *kin, uint64_t *kout,
+                              const uint32_t *vin, uint32_t *vout, size_t n, int endBit, cudaStream_t s);
+size_t cub_scan_u32_temp(size_t n);
+void   cub_exclusive_sum_u32(void *temp, size_t tempBytes, const uint32_t *in, uint32_t *out, size_t n, cudaStream_t s);
+size_t cub_scan_u64_temp(size_t n);
+void   cub_exclusive_sum_u32_to_u64(void *temp, size_t tempBytes, const uint32_t *in, uint64_t *out, size_t n, cudaStream_t s);
+
 struct Ctx {
   int device = 0;
   cudaStream_t stream = nullptr;
@@ -269,24 +283,39 @@ struct Ctx {
   std::vector<ProfEv> profEvents;
   // Grow-only scratch slots for the per-chunk working set of the mapping pipeline (hit keys, flags,
   // candidate arrays ...): after the first chunk nothing is allocated or freed inside the timed path.
-  std::map<int, DevBuf<uint8_t>> slots;
+  std::map<uint64_t, DevBuf<uint8_t>> slots;
+  // Temp storage of the CUB calls of the mapping path: one grow-only buffer serves them all, because every such call is
+  // enqueued on `stream` and its temp storage is dead once the call has run in stream order (a buffer that grows goes
+  // back to the caching allocator on `stream`, which is stream-ordered too).
+  DevBuf<uint8_t> cubTemp;
   // kernel function attributes (dynamic shared memory limit, carve-out) are per DEVICE: remember per context what has
   // been set, so that a process driving several GPUs (the C++ CLI: one thread + context per GPU) sets them on each
   std::map<const void *, bool> attrDone;
   bool first_time(const void *key) { bool &d = attrDone[key]; const bool f = !d; d = true; return f; }
-  template <typename T> View<T> view(int id, size_t n)
+  template <typename T> View<T> view(uint64_t id, size_t n)
   {
     DevBuf<uint8_t> &b = slots[id];
     const size_t bytes = (n ? n : 1) * sizeof(T);
     if (b.n < bytes) b.alloc(bytes + bytes / 8 + 256, stream);
     View<T> v; v.p = (T *)b.p; v.n = n; return v;
   }
+  void *cub_temp(size_t bytes) { if (cubTemp.n < bytes) cubTemp.alloc(bytes + bytes / 8 + 256, stream); return cubTemp.p; }
+  // exclusive sums and radix sorts on `stream`
+  void scan(const uint32_t *in, uint32_t *out, size_t n) { size_t b = cub_scan_u32_temp(n); cub_exclusive_sum_u32(cub_temp(b), b, in, out, n, stream); }
+  void scan(const uint32_t *in, unsigned long long *out, size_t n)
+  { size_t b = cub_scan_u64_temp(n); cub_exclusive_sum_u32_to_u64(cub_temp(b), b, in, (uint64_t *)out, n, stream); }
+  void sort_pairs(const uint32_t *kin, uint32_t *kout, const uint32_t *vin, uint32_t *vout, size_t n, int endBit)
+  { size_t b = cub_sort_pairs_u32_temp(n); cub_sort_pairs_u32(cub_temp(b), b, kin, kout, vin, vout, n, endBit, stream); }
+  void sort_pairs(const unsigned long long *kin, unsigned long long *kout, const uint32_t *vin, uint32_t *vout, size_t n, int endBit)
+  { size_t b = cub_sort_pairs_u64_u32_temp(n); cub_sort_pairs_u64_u32(cub_temp(b), b, (const uint64_t *)kin, (uint64_t *)kout, vin, vout, n, endBit, stream); }
+  void sort_keys(const unsigned long long *kin, unsigned long long *kout, size_t n, int endBit)
+  { size_t b = cub_sort_keys_u64_temp(n); cub_sort_keys_u64(cub_temp(b), b, (const uint64_t *)kin, (uint64_t *)kout, n, 0, endBit, stream); }
 };
-#ifndef BANI_FILE_TAG
-#define BANI_FILE_TAG 0
-#endif
+
+constexpr uint64_t fnv1a(const char *s, uint64_t h = 0xcbf29ce484222325ull)
+{ return *s ? fnv1a(s + 1, (h ^ (unsigned char)*s) * 0x100000001b3ull) : h; }
 // one scratch slot per (source file, source line): never put two BANI_SCRATCH on one line
-#define BANI_SLOT_ID ((BANI_FILE_TAG << 20) | __LINE__)
+#define BANI_SLOT_ID (::std::integral_constant<uint64_t, ::bani::fnv1a(__FILE__) ^ (uint64_t)__LINE__>::value)
 #define BANI_SCRATCH(T, name, count) ::bani::View<T> name = ctx->view<T>(BANI_SLOT_ID, (count))
 
 // RAII stage timer: records an event pair around a stage when profiling is on.
@@ -418,6 +447,24 @@ QSketch *qsketch_merge(Ctx *ctx, const QSketch *const *sketches, int32_t n);
 void qsketch_map(Ctx *ctx, const Index *ix, const QSketch *const *sketches, int32_t nSketches,
                  bool wantRows, bool wantCgi, MapOutput &out, bool wantFrags = false);
 
+// cgi.cu : stage H, the per-pair identity reduction of the mapping rows of a piece.  CgiState lives for one qsketch_map
+// call: the 2-way bin table, its touched flags per (query, genome) and the last contig of every genome.
+struct CgiState {
+  const Index *ix; bool frags;                  // frags: 8-byte bins that also identify the winning fragment, else 4-byte
+  uint64_t qMax = 0, tableQ = 0;                // queries the bin table may hold / holds (per pass over the rows)
+  DevBuf<uint8_t> table; DevBuf<uint8_t> touched; DevBuf<int32_t> gce;
+  CgiState(Ctx *ctx, const Index *ix, bool frags);
+  uint64_t bin_bytes() const { return frags ? 8 : 4; }
+};
+// Results in query-slot space: dense (count, identity) tables [slot][genome] or sparse pairs (qryGenomeId = slot), and
+// when CgiState::frags the 2-way winners (qryGenomeId = slot)
+struct CgiResult {
+  std::vector<int32_t> count; std::vector<float> ident; std::vector<bani_cgi_result> pairs; std::vector<bani_frag_mapping> frags;
+};
+// the R mapping rows of a piece in (fragment, candidate) order, the fragment of each row, the query slot (0 .. nQ) of each fragment
+void cgi_piece(Ctx *ctx, CgiState &cs, const bani_mapping *rows, const int32_t *rFrag, uint32_t R, const int32_t *fragQuery, int nQ,
+               uint64_t *pp, CgiResult &res);
+
 // hits.cu : per-fragment gather + shared-memory sort + L1 candidate regions
 static constexpr unsigned long long FRAG_L1_MAX = 8192;   // hits per fragment handled inside one CTA
 static constexpr int FRAG_NCLASS = 13;                    // size classes: 256 * {1,2,3,4,5,6,7,8,10,12,16,24,32} hits
@@ -448,19 +495,6 @@ void cand_compact(Ctx *ctx, const uint32_t *segStart, const unsigned long long *
 void synth_genome(Ctx *ctx, uint64_t seed, uint32_t ancestor, uint32_t strain, uint32_t ppm,
                   int64_t len, uint8_t *hostOut);
 
-// CUB-backed primitives (cubops.cu; kept in one TU because CUB compiles slowly)
-size_t cub_sort_pairs_u32_temp(size_t n);
-void   cub_sort_pairs_u32(void *temp, size_t tempBytes, const uint32_t *kin, uint32_t *kout,
-                          const uint32_t *vin, uint32_t *vout, size_t n, int endBit, cudaStream_t s);
-size_t cub_sort_keys_u64_temp(size_t n);
-void   cub_sort_keys_u64(void *temp, size_t tempBytes, const uint64_t *kin, uint64_t *kout, size_t n,
-                         int beginBit, int endBit, cudaStream_t s);
-size_t cub_sort_pairs_u64_u32_temp(size_t n);
-void   cub_sort_pairs_u64_u32(void *temp, size_t tempBytes, const uint64_t *kin, uint64_t *kout,
-                              const uint32_t *vin, uint32_t *vout, size_t n, int endBit, cudaStream_t s);
-size_t cub_scan_u32_temp(size_t n);
-void   cub_exclusive_sum_u32(void *temp, size_t tempBytes, const uint32_t *in, uint32_t *out, size_t n, cudaStream_t s);
-size_t cub_scan_u64_temp(size_t n);
-void   cub_exclusive_sum_u32_to_u64(void *temp, size_t tempBytes, const uint32_t *in, uint64_t *out, size_t n, cudaStream_t s);
+inline unsigned nblk(uint64_t n, int t = 256) { return (unsigned)((n + t - 1) / t); }    // blocks of t threads for n items
 
 } // namespace bani

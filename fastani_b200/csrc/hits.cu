@@ -19,12 +19,9 @@
 //               area addressed by the fragment's global hit offset (a fragment never has more regions than hits)
 // Fragments are binned by hit count into 13 size classes (256 ... 8192 hits per CTA, frag_class_items); larger
 // ones (many near-identical references) stay on the device-wide sort path in map.cu.
-#define BANI_FILE_TAG 1
 #include "common.cuh"
 
 namespace bani {
-
-static inline unsigned nblk(uint64_t n, int t = 256) { return (unsigned)((n + t - 1) / t); }
 
 __global__ void frag_classify_kernel(const uint32_t *segStart, const unsigned long long *hitOff, int32_t F,
                                      uint32_t *candCount, uint32_t *fragClass, uint32_t *classCount, uint32_t *classList, unsigned long long maxFast)

@@ -21,8 +21,6 @@
 
 namespace bani {
 
-static inline unsigned nblk(uint64_t n, int t = 256) { return (unsigned)((n + t - 1) / t); }
-
 __global__ void iota_kernel(uint32_t *v, uint64_t n)
 {
   uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;

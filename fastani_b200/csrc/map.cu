@@ -1,9 +1,8 @@
-// map.cu -- HP2: query mapping (+ the per-pair identity reduction that consumes it).
+// map.cu -- HP2: query mapping, stages A..G, and the piece loop that runs stages C..H.
 //
 // Replaces skch::Map::mapQuery / doL1Mapping / computeL1CandidateRegions / doL2Mapping /
 // computeL2MappedRegions (src/map/include/computeMap.hpp:112-497) with SlideMapper
-// (slidingMap.hpp) and MIIteratorL2 (MIIteratorL2.hpp), and cgi::computeCGI
-// (src/cgi/include/computeCoreIdentity.hpp:166-298).
+// (slidingMap.hpp) and MIIteratorL2 (MIIteratorL2.hpp).
 //
 // The reference maps one fragment at a time.  Here a batch of query genomes is cut into
 // fragments and every stage runs over ALL fragments (or all hits / all candidates) of a piece
@@ -14,7 +13,7 @@
 //   A' from index  for queries that are genomes of the index: the same multiset read from the
 //                  index's contig-level records + validity bitmap, no second hashing
 //   B  sort/unique per fragment: sorted unique hashes Q, s = |Q| (computeMap.hpp:268-276), packed
-//   --- map phase (qsketch_map) ---
+//   --- map phase (qsketch_map: one map_piece per piece, one host function per stage) ---
 //   C  lookup      Q -> bucket directory -> unique keys -> position lists (:283-299)
 //   D+E hits, L1   per fragment in one CTA (hits.cu): gather, sort by record index (monotone in
 //                  (seqId, wpos), i.e. the sort of :320), candidate regions of :322-352 as a LOCAL
@@ -28,8 +27,7 @@
 //                  sweep (each event moves t* by at most one)
 //   G  report      identity / upper bound from the (s, shared) table, filter >= cutoff (:375-384),
 //                  rows in (fragment, candidate) order == callback order of reportL2Mappings
-//   H  CGI         1-way best per (fragment, genome); 2-way best per (ref contig, position bin) via
-//                  atomicMax on a dense bin table; ordered float32 sum per genome pair
+//   H  CGI         the per-pair identity reduction of cgi::computeCGI                      cgi.cu
 #include "common.cuh"
 #include "cgi_rows.hpp"
 #include <algorithm>
@@ -37,8 +35,6 @@
 #include <deque>
 
 namespace bani {
-
-static inline unsigned nblk(uint64_t n, int t = 256) { return (unsigned)((n + t - 1) / t); }
 
 // ------------------------------------------------------------------ B: per-fragment sort + unique
 static constexpr int SU_THREADS = 128;
@@ -796,211 +792,6 @@ __global__ void rows_kernel(const RepArgs a, const uint32_t *keep, const uint32_
   if (rFrag) rFrag[keepScan[c]] = f;
 }
 
-// ------------------------------------------------------------------ H: CGI on the device
-struct CgiArgs {
-  const bani_mapping *rows; const int32_t *rFrag; uint32_t R;
-  const int32_t *fragQuery;            // chunk-local query slot of a fragment
-  const int32_t *contigGenome; const uint32_t *contigBinOff;
-  int fragLen; unsigned long long totalBins; int nGenomes;
-  uint32_t *table;                     // [querySlot - qLo][totalBins] float bits, 0 = empty
-  uint8_t *touched;                    // [querySlot - qLo][nGenomes]
-  int qLo, qHi;                        // query slots of the piece handled by this pass
-};
-
-// 1-way: best row of each (fragment, genome) by (identity, refSeqId, refStartPos) (cgid_types.hpp:31-39,
-// computeCoreIdentity.hpp:214-231): true if no other row of fragment f (row i, identity id) on genome g beats row i
-__device__ __forceinline__ bool cgi_one_way_winner(const CgiArgs &a, uint32_t i, int f, int g, float id)
-{
-  // rows of a fragment are contiguous and ordered by (refSeqId, refStartPos): a later row wins ties
-  for (uint32_t j = i + 1; j < a.R && a.rFrag[j] == f && a.contigGenome[a.rows[j].refSeqId] == g; j++)
-    if (a.rows[j].nucIdentity >= id) return false;
-  for (uint32_t j = i; j-- > 0 && a.rFrag[j] == f && a.contigGenome[a.rows[j].refSeqId] == g;)
-    if (a.rows[j].nucIdentity > id) return false;
-  return true;
-}
-
-__device__ __forceinline__ unsigned long long cgi_bin(const CgiArgs &a, const bani_mapping &r)
-{
-  return a.contigBinOff[r.refSeqId] + (uint32_t)(r.refStartPos / (a.fragLen - 20));
-}
-
-// 2-way: best identity per (ref contig, position bin) (:237-254)
-__global__ void cgi_scatter_kernel(const CgiArgs a)
-{
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= a.R) return;
-  const int f = a.rFrag[i];
-  const int q = a.fragQuery[f];
-  if (q < a.qLo || q >= a.qHi) return;
-  const bani_mapping r = a.rows[i];
-  const int g = a.contigGenome[r.refSeqId];
-  if (!cgi_one_way_winner(a, i, f, g, r.nucIdentity)) return;
-  atomicMax(a.table + (unsigned long long)(q - a.qLo) * a.totalBins + cgi_bin(a, r), __float_as_uint(r.nucIdentity));
-  a.touched[(size_t)(q - a.qLo) * a.nGenomes + g] = 1;
-}
-
-// Fragment-row mode of stage H (bani_map_cgi_sketch_frags): each bin holds the 64-bit key (identity bits << 32 | querySeqId)
-// of its winner.  Every row of one table row and bin has the same query and genome, and positive floats order as their
-// bits, so the 64-bit maximum is the best identity and, among equal identities, the largest querySeqId: the last element
-// of computeCGI's stable sort over the 1-way list, which is ordered by (genome, querySeqId) (computeCoreIdentity.hpp:237-254).
-struct CgiFragArgs {
-  unsigned long long *table;           // [querySlot - qLo][totalBins] keys, 0 = empty
-  uint8_t *win;                        // per row: 1-way winner of this pass
-  unsigned long long *key; uint32_t *row; uint32_t *count;   // emitted 2-way winners: (query slot << 32 | global bin), row
-};
-
-__device__ __forceinline__ unsigned long long cgi_frag_key(const bani_mapping &r)
-{
-  return ((unsigned long long)__float_as_uint(r.nucIdentity) << 32) | (uint32_t)r.querySeqId;
-}
-
-__global__ void cgi_scatter_frag_kernel(const CgiArgs a, const CgiFragArgs f)
-{
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= a.R) return;
-  const int fr = a.rFrag[i];
-  const int q = a.fragQuery[fr];
-  const bani_mapping r = a.rows[i];
-  const int g = a.contigGenome[r.refSeqId];
-  const bool w = q >= a.qLo && q < a.qHi && cgi_one_way_winner(a, i, fr, g, r.nucIdentity);
-  f.win[i] = w;
-  if (!w) return;
-  atomicMax(f.table + (unsigned long long)(q - a.qLo) * a.totalBins + cgi_bin(a, r), cgi_frag_key(r));
-  a.touched[(size_t)(q - a.qLo) * a.nGenomes + g] = 1;
-}
-
-// the 1-way winners that hold their bin's key: one per non-empty bin, appended in any order (sorted afterwards)
-__global__ void cgi_emit_kernel(const CgiArgs a, const CgiFragArgs f)
-{
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= a.R || !f.win[i]) return;
-  const bani_mapping r = a.rows[i];
-  const int q = a.fragQuery[a.rFrag[i]];
-  const unsigned long long bin = cgi_bin(a, r);
-  if (f.table[(unsigned long long)(q - a.qLo) * a.totalBins + bin] != cgi_frag_key(r)) return;
-  const uint32_t o = atomicAdd(f.count, 1u);
-  f.key[o] = ((unsigned long long)q << 32) | bin;
-  f.row[o] = i;
-}
-
-// sorted (query slot, bin) keys -> records; qryGenomeId holds the piece-local query slot until the host maps it
-__global__ void cgi_frag_gather_kernel(const bani_mapping *rows, const unsigned long long *key, const uint32_t *row, uint32_t n,
-                                       bani_frag_mapping *out)
-{
-  uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
-  if (j >= n) return;
-  const bani_mapping r = rows[row[j]];
-  bani_frag_mapping m;
-  m.qryGenomeId = (int32_t)(key[j] >> 32); m.querySeqId = r.querySeqId; m.refSeqId = r.refSeqId; m.refStartPos = r.refStartPos;
-  m.identity = r.nucIdentity;
-  out[j] = m;
-}
-
-// ordered float32 sum over the bins of one (query, genome) pair (computeCoreIdentity.hpp:267-297);
-// clears what it read so the table is all-zero again for the next chunk.  The identity is the high word of a 64-bit key.
-template <typename T>
-__device__ __forceinline__ void cgi_sum_pair(T *table, uint8_t *touched, const uint32_t *contigBinOff, const int32_t *genomeContigEnd,
-                                             unsigned long long totalBins, int nGenomes, int nQ, int32_t *oCount, float *oIdent)
-{
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= (uint32_t)nQ * (uint32_t)nGenomes) return;
-  const int q = i / nGenomes, g = i % nGenomes;
-  int32_t cnt = 0; float sum = 0.0f;
-  if (touched[i]) {
-    touched[i] = 0;
-    const uint32_t b0 = contigBinOff[g ? genomeContigEnd[g - 1] : 0], b1 = contigBinOff[genomeContigEnd[g]];
-    T *row = table + (unsigned long long)q * totalBins;
-    for (uint32_t b = b0; b < b1; b++) {
-      const T v = row[b];
-      if (v) { sum += __uint_as_float((uint32_t)(v >> (8 * sizeof(T) - 32))); cnt++; row[b] = 0; }
-    }
-  }
-  oCount[i] = cnt; oIdent[i] = cnt ? sum / cnt : 0.0f;
-}
-
-__global__ void cgi_sum_kernel(uint32_t *table, uint8_t *touched, const uint32_t *contigBinOff, const int32_t *genomeContigEnd,
-                               unsigned long long totalBins, int nGenomes, int nQ, int32_t *oCount, float *oIdent)
-{
-  cgi_sum_pair(table, touched, contigBinOff, genomeContigEnd, totalBins, nGenomes, nQ, oCount, oIdent);
-}
-
-__global__ void cgi_sum_frag_kernel(unsigned long long *table, uint8_t *touched, const uint32_t *contigBinOff, const int32_t *genomeContigEnd,
-                                    unsigned long long totalBins, int nGenomes, int nQ, int32_t *oCount, float *oIdent)
-{
-  cgi_sum_pair(table, touched, contigBinOff, genomeContigEnd, totalBins, nGenomes, nQ, oCount, oIdent);
-}
-
-// Sparse stage H: the same reduction from the rows of a piece, with no table over (query, bin) or (query, genome).  Used
-// for pieces whose dense output would dwarf their rows (many small genomes).  Every row gets a key: 1-way winners
-// (query slot << binBits | global bin), the others the sentinel (nQ << binBits), which sorts after every real key.  So a
-// radix sort over the significant bits of all R rows compacts the winners to the front without a host-side count.
-__global__ void cgi_sparse_key_kernel(const CgiArgs a, int binBits, int nQ, unsigned long long *key, uint32_t *row)
-{
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= a.R) return;
-  const int f = a.rFrag[i];
-  const int q = a.fragQuery[f];
-  const bani_mapping r = a.rows[i];
-  const int g = a.contigGenome[r.refSeqId];
-  const bool w = cgi_one_way_winner(a, i, f, g, r.nucIdentity);
-  key[i] = w ? ((unsigned long long)q << binBits) | cgi_bin(a, r) : (unsigned long long)nQ << binBits;
-  row[i] = i;
-}
-
-// 1 where a run of equal winner keys -- one (query slot, bin) -- starts; n + 1 flags, the last 0 (exclusive scan -> count)
-__global__ void cgi_sparse_bin_head_kernel(const unsigned long long *key, uint32_t n, unsigned long long sentinel, uint32_t *head)
-{
-  uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
-  if (j > n) return;
-  head[j] = j < n && key[j] < sentinel && (j == 0 || key[j] != key[j - 1]);
-}
-
-// One thread per bin: its 2-way winner is the row with the largest 64-bit key (identity bits << 32 | querySeqId) -- what
-// the dense path's atomicMax keeps; the pair is unique within a bin, so the winning row is deterministic.  Writes the bin
-// as (query slot << 32 | global bin) with its row, and flags the bins that start a (query slot, genome) pair: bins of a
-// genome are contiguous in the global bin order, so the pairs are runs of the sorted bins.
-__global__ void cgi_sparse_bin_max_kernel(const CgiArgs a, const unsigned long long *key, const uint32_t *row, uint32_t n, int binBits,
-                                          const uint32_t *head, const uint32_t *binIdx,
-                                          unsigned long long *binKey, uint32_t *binRow, uint32_t *pairHead)
-{
-  uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
-  if (j >= n || !head[j]) return;
-  const unsigned long long k = key[j];
-  uint32_t best = row[j];
-  unsigned long long bestV = cgi_frag_key(a.rows[best]);
-  for (uint32_t t = j + 1; t < n && key[t] == k; t++) {
-    const unsigned long long v = cgi_frag_key(a.rows[row[t]]);
-    if (v > bestV) { bestV = v; best = row[t]; }
-  }
-  const unsigned long long q = k >> binBits, bin = k & ((1ull << binBits) - 1);
-  const uint32_t b = binIdx[j];
-  binKey[b] = (q << 32) | bin;
-  binRow[b] = best;
-  const int g = a.contigGenome[a.rows[best].refSeqId];
-  pairHead[b] = j == 0 || (key[j - 1] >> binBits) != q || a.contigGenome[a.rows[row[j - 1]].refSeqId] != g;
-}
-
-// One thread per (query slot, genome) pair: the float32 sum of its bin winners' identities in ascending bin order, divided
-// by the count -- cgi_sum_pair's order and arithmetic, including its skipping of a bin whose value is 0.  Writes the pair
-// as a bani_cgi_result with the query slot in qryGenomeId (the host maps it), in (query slot, genome) order.
-__global__ void cgi_sparse_pair_kernel(const CgiArgs a, const unsigned long long *binKey, const uint32_t *binRow, const uint32_t *nBinsP,
-                                       const uint32_t *pairHead, const uint32_t *pairIdx, bool fragKeys, bani_cgi_result *out)
-{
-  uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
-  const uint32_t nBins = *nBinsP;
-  if (b >= nBins || !pairHead[b]) return;
-  int32_t cnt = 0; float sum = 0.0f;
-  for (uint32_t t = b; t < nBins && (t == b || !pairHead[t]); t++) {
-    const bani_mapping &r = a.rows[binRow[t]];
-    const unsigned long long v = fragKeys ? cgi_frag_key(r) : (unsigned long long)__float_as_uint(r.nucIdentity);
-    if (v) { sum += r.nucIdentity; cnt++; }
-  }
-  bani_cgi_result o;
-  o.refGenomeId = a.contigGenome[a.rows[binRow[b]].refSeqId]; o.qryGenomeId = (int32_t)(binKey[b] >> 32);
-  o.countSeq = cnt; o.totalQueryFragments = 0; o.identity = cnt ? sum / cnt : 0.0f;
-  out[pairIdx[b]] = o;
-}
-
 // ------------------------------------------------------------------ host orchestration
 __global__ void scount_present_kernel(const int32_t *sCount, int32_t F, int smax, uint32_t *present)
 {
@@ -1140,9 +931,6 @@ __global__ void compact_sketch_kernel(const uint32_t *raw, const uint32_t *rawSt
 // fragments per piece: the working set of a piece (hit staging, L2 event streams: ~25 GB for 2^18 fragments of config 3)
 // must fit an 80 GB device next to the index of a 1000-genome shard (~32 GB).  The switch frags_per_piece lowers it.
 static constexpr uint64_t FRAG_MAX = 1u << 18;
-// stage H takes the sparse path when a piece's dense (query, genome) output exceeds both its rows and this many entries
-// (32 MB of count + identity): below it the dense tables cost less than the sparse path's sort (DESIGN.md section 6)
-static constexpr uint64_t CGI_SPARSE_MIN_PAIRS = 1u << 22;
 static uint64_t frags_per_piece(const Ctx *ctx) { return std::min<uint64_t>(FRAG_MAX, (uint64_t)std::max(1ll, ctx->flags.fragsPerPiece)); }
 
 // A query as the sketch stage sees it: a contig-length table plus either the packed bases (stage A) or the first contig
@@ -1264,9 +1052,7 @@ static QSketch *qsketch_build(Ctx *ctx, const std::vector<QuerySrc> &srcs, const
         frag_ref_range_kernel<<<nblk((uint64_t)F + 1), 256, 0, st>>>(d_src.p, (int32_t)src.size(), F, fragLen, k, w, hint->wpos.p, hint->contigRecOff.p,
                                                                      hint->validBits.p, hint->contigBitBase.p, rFirst.p, rCnt.p);
         ctx->launches++;
-        { size_t tb = cub_scan_u32_temp((size_t)F + 1);
-          BANI_SCRATCH(uint8_t, tmp, tb);
-          cub_exclusive_sum_u32(tmp.p, tb, rCnt.p, rawStart.p, (size_t)F + 1, st); }
+        ctx->scan(rCnt.p, rawStart.p, (size_t)F + 1);
         uint32_t t32 = 0;
         BANI_CUDA(cudaMemcpyAsync(&t32, rawStart.p + F, 4, cudaMemcpyDeviceToHost, st));
         BANI_CUDA(cudaStreamSynchronize(st));
@@ -1308,9 +1094,7 @@ static QSketch *qsketch_build(Ctx *ctx, const std::vector<QuerySrc> &srcs, const
         BANI_SCRATCH(uint32_t, cnt1, (size_t)F + 1);
         BANI_CUDA(cudaMemcpyAsync(cnt1.p, pc->sCount.p, 4 * (size_t)F, cudaMemcpyDeviceToDevice, st));
         BANI_CUDA(cudaMemsetAsync(cnt1.p + F, 0, 4, st));
-        size_t tb = cub_scan_u32_temp((size_t)F + 1);
-        BANI_SCRATCH(uint8_t, tmp, tb);
-        cub_exclusive_sum_u32(tmp.p, tb, cnt1.p, pc->segStart.p, (size_t)F + 1, st);
+        ctx->scan(cnt1.p, pc->segStart.p, (size_t)F + 1);
         int hflags[2]; uint32_t t2 = 0;
         BANI_CUDA(cudaMemcpyAsync(hflags, d_flags.p, 8, cudaMemcpyDeviceToHost, st));
         BANI_CUDA(cudaMemcpyAsync(&t2, pc->segStart.p + F, 4, cudaMemcpyDeviceToHost, st));
@@ -1575,496 +1359,381 @@ void map_queries(Ctx *ctx, const Index *ix, const Genome *const *queries, int32_
   ctx->mark("map: query sketches freed");
 }
 
+// ------------------------------------------------------------------ stages C..G of one piece
+// What a stage hands to the next.  The Views are scratch slots of the function that fills them: each of those
+// functions runs once per piece, so the arrays stay valid until the piece is done.
+struct Hits {                                   // C: index hits of the T query hashes (T + 1 entries, the last one 0)
+  View<uint32_t> lo, cnt; View<unsigned long long> off;     // first posIdx entry, count, exclusive scan of the counts
+  unsigned long long N = 0;
+  DevBuf<unsigned long long> walkCtr;           // probes that walked the sorted keys (flags.countPaths)
+};
+struct Cands { View<int32_t> frag, seq, start, end; uint32_t C = 0; };     // D+E: compact L1 candidate regions
+struct Scores {                                 // F: best window of every candidate, window evaluations (n2, on the device)
+  View<int32_t> pos, best; View<unsigned long long> n2;
+  size_t idEv = (size_t)-1; double evBytes = 0; // timer of l2_events: its bytes are set once n2 is known
+};
+struct Rows { View<bani_mapping> rows; DevBuf<int32_t> frag; uint32_t R = 0; };   // G: rows past the cutoff, fragment of each
+
+// C: lookup.  N and the walk counters come back behind one synchronisation.
+static void lookup(Ctx *ctx, const Index *ix, const QPiece &pc, uint64_t *pp, Hits &h)
+{
+  cudaStream_t st = ctx->stream;
+  const uint64_t T = pc.T;
+  BANI_SCRATCH(uint32_t, hitLo, T + 1);
+  BANI_SCRATCH(uint32_t, hitCnt, T + 1);
+  BANI_SCRATCH(unsigned long long, hitOff, T + 1);
+  h.lo = hitLo; h.cnt = hitCnt; h.off = hitOff;
+  if (ctx->flags.countPaths) { h.walkCtr.alloc(2, st); BANI_CUDA(cudaMemsetAsync(h.walkCtr.p, 0, 16, st)); }
+  { Stage sg(ctx, "lookup", 12.0 * T);
+    // the membership filter pays when most probes miss: not for queries that are genomes of this very index
+    const bool useFilt = ix->filt.p && pc.memberOf != ix->uid;
+    lookup_kernel<<<nblk(T + 1), 256, 0, st>>>(pc.fragHash.p, (uint32_t)T, ix->tab.p, (1u << ix->tabBits) - 1u, ix->ukeys.p, ix->uoff.p,
+                                               ix->dir.p, ix->dirBits, useFilt ? ix->filt.p : nullptr,
+                                               useFilt ? (uint32_t)((1ull << ix->filtBits) - 1ull) : 0u, hitLo.p, hitCnt.p, h.walkCtr.p);
+    ctx->launches++;
+    ctx->scan(hitCnt.p, hitOff.p, T + 1); }
+  BANI_CUDA(cudaMemcpyAsync(&h.N, hitOff.p + T, 8, cudaMemcpyDeviceToHost, st));
+  if (ctx->flags.countPaths) BANI_CUDA(cudaMemcpyAsync(pp + P_LOOKUP_WALK_SATURATED, h.walkCtr.p, 16, cudaMemcpyDeviceToHost, st));
+  BANI_CUDA(cudaStreamSynchronize(st));
+  ctx->mark("piece: lookup done");
+}
+
+// D+E for the fragments with more hits than one CTA takes: (fragment, record) keys, one radix sort, flags + scan + write.
+// The regions go to the staging area of l1_candidates, at the fragment's hit offset.
+static void l1_device_wide(Ctx *ctx, const Index *ix, const QPiece &pc, const Hits &h, const uint32_t *fragClass,
+                           int32_t *stSeq, int32_t *stStart, int32_t *stEnd, uint32_t *candCount)
+{
+  cudaStream_t st = ctx->stream;
+  const int32_t F = pc.F; const uint64_t T = pc.T;
+  BANI_SCRATCH(uint32_t, bigCnt, T + 1);
+  BANI_SCRATCH(unsigned long long, bigOff, T + 1);
+  mask_hits_kernel<<<nblk(T + 1), 256, 0, st>>>(pc.segStart.p, F, (uint32_t)T, h.cnt.p, fragClass, bigCnt.p); ctx->launches++;
+  ctx->scan(bigCnt.p, bigOff.p, T + 1);
+  unsigned long long NB = 0;
+  BANI_CUDA(cudaMemcpyAsync(&NB, bigOff.p + T, 8, cudaMemcpyDeviceToHost, st));
+  BANI_CUDA(cudaStreamSynchronize(st));
+  BANI_SCRATCH(unsigned long long, keysA, NB);
+  BANI_SCRATCH(unsigned long long, keysB, NB);
+  { Stage sg(ctx, "hit_gather", 12.0 * NB);
+    gather_kernel<<<nblk(T), 256, 0, st>>>(pc.segStart.p, F, (uint32_t)T, h.lo.p, bigCnt.p, bigOff.p, ix->posIdx.p, keysA.p); ctx->launches++; }
+  int fbits = 1; while ((1ll << fbits) < F) fbits++;
+  { Stage sg(ctx, "hit_sort", 16.0 * NB);
+    ctx->sort_keys(keysA.p, keysB.p, NB, 32 + fbits); }
+  L1Args la; la.keys = keysB.p; la.N = NB; la.segStart = pc.segStart.p; la.hitOff = bigOff.p; la.sCount = pc.sCount.p;
+  la.minHits = ctx->d_minHits.p; la.recSeq = ix->seqId.p; la.recWpos = ix->wpos.p; la.fragLen = ctx->prm.frag_len;
+  BANI_SCRATCH(uint32_t, head, NB + 1);
+  BANI_SCRATCH(uint32_t, headScan, NB + 1);
+  { Stage sg(ctx, "l1_flags", 8.0 * NB);
+    l1_flag_kernel<<<nblk(NB + 1), 256, 0, st>>>(la, head.p);
+    ctx->launches++;
+    ctx->scan(head.p, headScan.p, NB + 1); }
+  uint32_t CB = 0;
+  BANI_CUDA(cudaMemcpyAsync(&CB, headScan.p + NB, 4, cudaMemcpyDeviceToHost, st));
+  BANI_CUDA(cudaStreamSynchronize(st));
+  if (CB == 0) return;
+  BANI_SCRATCH(int32_t, bFrag, CB);
+  BANI_SCRATCH(int32_t, bSeq, CB);
+  BANI_SCRATCH(int32_t, bStart, CB);
+  BANI_SCRATCH(int32_t, bEnd, CB);
+  Stage sg(ctx, "l1_write", 8.0 * NB);
+  l1_write_kernel<<<nblk(NB), 256, 0, st>>>(la, head.p, headScan.p, bFrag.p, bSeq.p, bStart.p, bEnd.p); ctx->launches++;
+  cand_stage(ctx, bFrag.p, bSeq.p, bStart.p, bEnd.p, CB, pc.segStart.p, h.off.p, stSeq, stStart, stEnd, candCount);
+}
+
+// D+E: hits -> L1 candidate regions.  Fragments with at most FRAG_L1_MAX hits are handled by one CTA each (hits.cu), the
+// others by l1_device_wide.  Both write their regions to a staging area addressed by the fragment's hit offset; a scan +
+// copy makes them dense.
+static void l1_candidates(Ctx *ctx, const Index *ix, const QPiece &pc, const Hits &h, uint64_t *pp, Cands &cd)
+{
+  cudaStream_t st = ctx->stream;
+  const int32_t F = pc.F; const unsigned long long N = h.N;
+  BANI_SCRATCH(uint32_t, candCount, (size_t)F + 1);
+  BANI_SCRATCH(uint32_t, candOff, (size_t)F + 1);
+  BANI_SCRATCH(uint32_t, fragClass, F);
+  BANI_SCRATCH(uint32_t, classList, (size_t)FRAG_NCLASS * F);
+  BANI_SCRATCH(uint32_t, classCount, FRAG_NCLASS + 2);
+  BANI_SCRATCH(int32_t, stSeq, N);
+  BANI_SCRATCH(int32_t, stStart, N);
+  BANI_SCRATCH(int32_t, stEnd, N);
+  const long long maxFast = std::max(0ll, std::min(ctx->flags.fragL1Max, (long long)FRAG_L1_MAX));
+  uint32_t hClass[FRAG_NCLASS + 2];
+  { Stage sg(ctx, "frag_l1", 12.0 * N);                // 4 B list entry + 8 B (seqId, wpos) per hit
+    frag_classify(ctx, pc.segStart.p, h.off.p, F, candCount.p, fragClass.p, classCount.p, classList.p, (unsigned long long)maxFast);
+    BANI_CUDA(cudaMemcpyAsync(hClass, classCount.p, sizeof hClass, cudaMemcpyDeviceToHost, st));
+    BANI_CUDA(cudaStreamSynchronize(st));
+    for (int i = 0; i <= FRAG_NCLASS; i++) pp[P_L1_CLASS0 + i] += hClass[i];
+    FragL1Args fa; fa.segStart = pc.segStart.p; fa.sCount = pc.sCount.p; fa.F = F; fa.hitLo = h.lo.p; fa.hitCnt = h.cnt.p; fa.hitOff = h.off.p;
+    fa.posIdx = ix->posIdx.p; fa.recPos = ix->pos8.p; fa.minHits = ctx->d_minHits.p; fa.fragLen = ctx->prm.frag_len;
+    fa.keyBits = 1; while (fa.keyBits < 32 && (1ull << fa.keyBits) < ix->M) fa.keyBits++;
+    fa.stSeq = stSeq.p; fa.stStart = stStart.p; fa.stEnd = stEnd.p; fa.candCount = candCount.p;
+    frag_l1_fast(ctx, fa, classList.p, hClass); }
+  if (hClass[FRAG_NCLASS] > 0) l1_device_wide(ctx, ix, pc, h, fragClass.p, stSeq.p, stStart.p, stEnd.p, candCount.p);
+  BANI_CUDA(cudaMemsetAsync(candCount.p + F, 0, 4, st));
+  ctx->scan(candCount.p, candOff.p, (size_t)F + 1);
+  BANI_CUDA(cudaMemcpyAsync(&cd.C, candOff.p + F, 4, cudaMemcpyDeviceToHost, st));
+  BANI_CUDA(cudaStreamSynchronize(st));
+  if (cd.C == 0) return;
+  BANI_SCRATCH(int32_t, cFrag, cd.C);
+  BANI_SCRATCH(int32_t, cSeq, cd.C);
+  BANI_SCRATCH(int32_t, cStart, cd.C);
+  BANI_SCRATCH(int32_t, cEnd, cd.C);
+  cd.frag = cFrag; cd.seq = cSeq; cd.start = cStart; cd.end = cEnd;
+  cand_compact(ctx, pc.segStart.p, h.off.p, F, candCount.p, candOff.p, stSeq.p, stStart.p, stEnd.p, cFrag.p, cSeq.p, cStart.p, cEnd.p);
+}
+
+// Fast path of F: candidates by descending event count (rank g -> warp g / 32, lane g % 32 of l2_seq_kernel), their
+// window-event streams, the sequential sweep.  Stops the l2_bounds timer before the events.  Returns
+// P_PIECE_SPLIT_EVENTS, with nothing launched past the scan of the group steps, when the event streams would not fit.
+static PathId l2_fast(Ctx *ctx, const QPiece &pc, L2PArgs &lp, uint32_t *cOff, Stage &sgb, uint64_t *pp, Scores &sc)
+{
+  cudaStream_t st = ctx->stream;
+  const int32_t F = pc.F; const uint32_t C = lp.C;
+  BANI_SCRATCH(uint32_t, skey, C);
+  BANI_SCRATCH(uint32_t, skey2, C);
+  BANI_SCRATCH(uint32_t, sval, C);
+  BANI_SCRATCH(uint32_t, perm, C);
+  l2_sortkey_kernel<<<nblk(C), 256, 0, st>>>(lp.cNEv, C, skey.p, sval.p); ctx->launches++;
+  ctx->sort_pairs(skey.p, skey2.p, sval.p, perm.p, C, 20);
+  lp.perm = perm.p;
+  // event streams, interleaved per warp: step k of lane l of warp G is the 32-byte slot (grpOff[G] + k) * 32 + l,
+  // so a warp reads 1 KB contiguous per step while every 32-byte sector still belongs to one candidate
+  const uint32_t nGrp = (C + 31) / 32;
+  BANI_SCRATCH(uint32_t, grpSteps, (size_t)nGrp + 1);
+  BANI_SCRATCH(unsigned long long, grpOff, (size_t)nGrp + 1);
+  l2_group_steps_kernel<<<nblk((uint64_t)nGrp + 1), 256, 0, st>>>(lp.cChunks, perm.p, C, nGrp, grpSteps.p); ctx->launches++;
+  ctx->scan(grpSteps.p, grpOff.p, (size_t)nGrp + 1);
+  unsigned long long totalGrpSteps = 0;
+  BANI_CUDA(cudaMemcpyAsync(&totalGrpSteps, grpOff.p + nGrp, 8, cudaMemcpyDeviceToHost, st));
+  BANI_CUDA(cudaStreamSynchronize(st));
+  const unsigned long long totalSteps = totalGrpSteps * 32;     // 32-byte slots
+  // the event streams of this piece would take more than a quarter of the device (small windows make many events per
+  // hit): map its halves instead, so that they fit beside the index
+  const double evLimit = ctx->flags.eventBytesPerPiece > 0 ? (double)ctx->flags.eventBytesPerPiece : 0.25 * (double)ctx->memTotal;
+  if ((double)totalSteps * 32.0 > evLimit && pc.nq > 1) return P_PIECE_SPLIT_EVENTS;
+  if (totalSteps > 0xfffffff0ull) fail(BANI_ERR_LIMIT, "query chunk schedules more than 2^36 window events");
+  BANI_SCRATCH(uint16_t, events, (size_t)totalSteps * 16 + 64);
+  lp.events = events.p; lp.grpOff = grpOff.p;
+  l2_stream_base_kernel<<<nblk(C), 256, 0, st>>>(perm.p, grpOff.p, C, cOff); ctx->launches++;
+  // CTA size of the events kernel by candidates per fragment (warp per candidate: no idle warps in small shards)
+  const int evNT = ((uint64_t)C >= 6ull * (uint64_t)F) ? 256 : ((uint64_t)C >= 3ull * (uint64_t)F) ? 128 : 64;
+  if (ctx->flags.countPaths) {
+    // candidates with window events, by the variant of l2_events_kernel that writes them
+    std::vector<uint32_t> nEv(C); std::vector<uint16_t> mb(C);
+    BANI_CUDA(cudaMemcpyAsync(nEv.data(), lp.cNEv, 4 * (size_t)C, cudaMemcpyDeviceToHost, st));
+    BANI_CUDA(cudaMemcpyAsync(mb.data(), lp.cMB, 2 * (size_t)C, cudaMemcpyDeviceToHost, st));
+    BANI_CUDA(cudaStreamSynchronize(st));
+    uint64_t withEv = 0, staged = 0;
+    for (uint32_t c = 0; c < C; c++) if (nEv[c]) { withEv++; staged += mb[c] != 0xFFFFu; }
+    pp[evNT == 256 ? P_L2_EVENTS_NT256 : evNT == 128 ? P_L2_EVENTS_NT128 : P_L2_EVENTS_NT64] += withEv;
+    pp[lp.nBuckets == L2E_BUCKETS ? P_L2_DIR4096 : P_L2_DIR1024] += withEv;
+    pp[P_L2_STAGED] += staged; pp[P_L2_DIRECT] += withEv - staged;
+  }
+  const size_t shmE = 4 * ((size_t)(evNT / 32) * (L2E_RING / 2) + (size_t)lp.sLimit + 4 + L2E_BUCKETS + 4 + 2) + 8 * ((size_t)lp.sLimit + 4) + 16;
+  const size_t shmS = (size_t)L2S_WARPS * lp.warpBytes;
+  if (shmE > (size_t)L2_SHM_BUDGET || shmS > (size_t)L2_SHM_BUDGET) fail(BANI_ERR_INTERNAL, "L2 shared-memory budget exceeded");
+  if (ctx->first_time((const void *)l2_seq_kernel)) {
+    BANI_CUDA(cudaFuncSetAttribute(l2_events_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, L2_SHM_BUDGET));
+    BANI_CUDA(cudaFuncSetAttribute(l2_events_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, L2_SHM_BUDGET));
+    BANI_CUDA(cudaFuncSetAttribute(l2_events_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, L2_SHM_BUDGET));
+    BANI_CUDA(cudaFuncSetAttribute(l2_seq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, L2_SHM_BUDGET));
+    BANI_CUDA(cudaFuncSetAttribute(l2_seq_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
+  }
+  sgb.stop();
+  { Stage sg(ctx, "l2_events"); sc.idEv = sg.id(); sc.evBytes = 32.0 * (double)totalSteps;
+    if (evNT == 256) l2_events_kernel<256><<<F, 256, shmE, st>>>(lp);
+    else if (evNT == 128) l2_events_kernel<128><<<F, 128, shmE, st>>>(lp);
+    else l2_events_kernel<64><<<F, 64, shmE, st>>>(lp);
+    ctx->launches++; }
+  { Stage sg(ctx, "l2_seq", sc.evBytes + 16.0 * C);       // the event codes in, {position, shared} out
+    l2_seq_kernel<<<nblk(C, L2S_WARPS * 32), L2S_WARPS * 32, shmS, st>>>(lp); ctx->launches++; }
+  return P_PIECE_MAPPED;
+}
+
+// F: L2.  Bounds of every candidate, the fast path where the index has the window links for it, the exact kernel for
+// what is left.  Returns P_PIECE_SPLIT_EVENTS when the piece's window events would not fit.
+static PathId l2_candidates(Ctx *ctx, const Index *ix, const QPiece &pc, const Cands &cd, uint64_t *pp, Scores &sc)
+{
+  cudaStream_t st = ctx->stream;
+  const int32_t F = pc.F; const uint32_t C = cd.C; const int smax = pc.smax;
+  const int k = ctx->prm.kmer_size, w = ctx->prm.window_size, fragLen = ctx->prm.frag_len;
+  const int cmw = fragLen - (w - 1) - (k - 1);         // computeMap.hpp:427
+  const bool countPaths = ctx->flags.countPaths != 0;
+  BANI_SCRATCH(int32_t, cPos, C);
+  BANI_SCRATCH(int32_t, cBest, C);
+  sc.pos = cPos; sc.best = cBest;
+  L2Args l2; l2.cFrag = cd.frag.p; l2.cSeq = cd.seq.p; l2.cStart = cd.start.p; l2.cEnd = cd.end.p; l2.C = C;
+  l2.fragHash = pc.fragHash.p; l2.segStart = pc.segStart.p; l2.sCount = pc.sCount.p;
+  l2.recHash = ix->hash.p; l2.recWpos = ix->wpos.p; l2.recLink = ix->link.p; l2.contigRecOff = ix->contigRecOff.p;
+  l2.fragLen = fragLen; l2.cmw = cmw; l2.smax = smax;
+  l2.stride = ((size_t)2 * (smax + 2) + smax + 15) / 16 * 16;
+  const unsigned blocks = (unsigned)std::min<uint64_t>((C + 63) / 64, (uint64_t)ctx->smCount * 16);
+  BANI_SCRATCH(uint8_t, scratch, (size_t)blocks * 64 * l2.stride);
+  BANI_SCRATCH(unsigned long long, d_n2, 1);
+  sc.n2 = d_n2;
+  BANI_CUDA(cudaMemsetAsync(d_n2.p, 0, 8, st));
+  l2.scratch = scratch.p; l2.cPos = cPos.p; l2.cBest = cBest.p; l2.onlyFlagged = 1;
+  Stage sgb(ctx, "l2_bounds", 12.0 * C);
+  BANI_SCRATCH(uint32_t, fragCandOff, (size_t)F + 1);
+  frag_cand_off_kernel<<<nblk((uint64_t)F + 1), 256, 0, st>>>(cd.frag.p, C, F, fragCandOff.p);
+  ctx->launches++;
+  L2PArgs lp; lp.cFrag = cd.frag.p; lp.cSeq = cd.seq.p; lp.cStart = cd.start.p; lp.cEnd = cd.end.p; lp.C = C;
+  lp.fragCandOff = fragCandOff.p; lp.fragHash = pc.fragHash.p; lp.segStart = pc.segStart.p; lp.sCount = pc.sCount.p;
+  lp.rec = ix->rec.p; lp.recWposSoA = ix->wpos.p; lp.contigRecOff = ix->contigRecOff.p; lp.fragLen = fragLen; lp.cmw = cmw;
+  lp.rec8 = ix->rec8.p; lp.recLink = ix->link.p; lp.blkMax = ix->blkMax.p; lp.stage = ctx->flags.l2Stage;
+  // fast path: needs the window links of the index (cmw >= 2) and ranks that fit the event code
+  // (and whose per-warp state fits the shared-memory budget of l2_seq_kernel: larger sketches take l2_kernel)
+  // (the switch l2_fast = 0 sends every candidate to l2_kernel)
+  lp.sLimit = (ctx->flags.l2Fast && cmw >= 2 && ix->cmw == cmw && ix->rec8.p) ? std::min(std::min(smax, L2_SMAX), L2_SHM_BUDGET / (L2S_WARPS * 32) - 2) : 0;
+  // bucket width near 0 ~ 2^32 / (s * w): minimizer hashes are minima of w hashes, density w/2^32 at 0
+  lp.nBuckets = ((uint64_t)C >= 8ull * (uint64_t)F) ? L2E_BUCKETS : 1024;      // few candidates per fragment: building a big directory is not worth it
+  { const int forced = ctx->flags.l2eBuckets;
+    if (forced == 1024 || forced == L2E_BUCKETS) lp.nBuckets = forced; }
+  { int sh = lp.nBuckets == L2E_BUCKETS ? 20 : 22; while (sh > 8 && ((uint64_t)std::max(smax, 1) * (uint64_t)w << sh) > ((1ull << 32) * (uint64_t)(L2E_BUCKETS / lp.nBuckets))) sh--; lp.shiftA = sh; }
+  lp.warpBytes = (uint32_t)(std::max(lp.sLimit, 1) + 1) * 32u;      // one state byte per rank 0..s and lane
+  BANI_SCRATCH(uint32_t, cB0, C);          // (one scratch slot per source line)
+  BANI_SCRATCH(uint32_t, cE0, C);
+  BANI_SCRATCH(uint32_t, cLast, C);
+  BANI_SCRATCH(uint32_t, cNEv, C);
+  BANI_SCRATCH(uint32_t, cChunks, (size_t)C + 1);
+  BANI_SCRATCH(uint32_t, cOff, (size_t)C + 1);
+  BANI_SCRATCH(uint16_t, cMB, (size_t)C + 1);
+  lp.cMB = cMB.p;
+  lp.cB0 = cB0.p; lp.cE0 = cE0.p; lp.cLast = cLast.p; lp.cNEv = cNEv.p; lp.cChunks = cChunks.p; lp.cOff = cOff.p;
+  lp.cPos = cPos.p; lp.cBest = cBest.p; lp.ctr_n2 = d_n2.p; lp.events = nullptr; lp.perm = nullptr;
+  l2_bounds_kernel<<<nblk((uint64_t)C + 1), 256, 0, st>>>(lp); ctx->launches++;
+  if (countPaths) pp[P_L2_EXACT_AT_BOUNDS] += count_exact(ctx, cBest.p, C);
+  if (lp.sLimit > 0 && l2_fast(ctx, pc, lp, cOff.p, sgb, pp, sc) == P_PIECE_SPLIT_EVENTS) return P_PIECE_SPLIT_EVENTS;
+  sgb.stop();
+  if (countPaths) pp[P_L2_EXACT_TOTAL] += count_exact(ctx, cBest.p, C);
+  // exact slow path for whatever the fast path flagged (counter overflow, very large sketches)
+  Stage sgs(ctx, "l2_exact");
+  l2_kernel<<<blocks, 64, 0, st>>>(l2); ctx->launches++;
+  return P_PIECE_MAPPED;
+}
+
+// G: report.  R and n2 come back behind one synchronisation; the rows go to *hostRows when it is given.
+static void report(Ctx *ctx, const QPiece &pc, const Cands &cd, const Scores &sc, bani_map_counters &ctr,
+                   std::vector<bani_mapping> *hostRows, Rows &rw)
+{
+  cudaStream_t st = ctx->stream;
+  const uint32_t C = cd.C;
+  RepArgs ra; ra.cFrag = cd.frag.p; ra.cSeq = cd.seq.p; ra.cPos = sc.pos.p; ra.cBest = sc.best.p; ra.C = C;
+  ra.sCount = pc.sCount.p; ra.fragSeqId = pc.fragSeqId.p; ra.rowOff = ctx->d_rowOff.p; ra.ident = ctx->d_ident.p;
+  ra.upper = ctx->d_upper.p; ra.pid = ctx->prm.perc_identity; ra.fragLen = ctx->prm.frag_len;
+  BANI_SCRATCH(uint32_t, keep, C + 1);
+  BANI_SCRATCH(uint32_t, keepScan, C + 1);
+  keep_flag_kernel<<<nblk(C + 1), 256, 0, st>>>(ra, keep.p);
+  ctx->launches++;
+  ctx->scan(keep.p, keepScan.p, C + 1);
+  unsigned long long n2 = 0;
+  BANI_CUDA(cudaMemcpyAsync(&rw.R, keepScan.p + C, 4, cudaMemcpyDeviceToHost, st));
+  BANI_CUDA(cudaMemcpyAsync(&n2, sc.n2.p, 8, cudaMemcpyDeviceToHost, st));
+  BANI_CUDA(cudaStreamSynchronize(st));
+  ctr.n2 += n2; ctr.mappings += rw.R;
+  ctx->mark("piece: L1 + L2 done");
+  Stage::set_bytes(ctx, sc.idEv, 16.0 * (double)n2 + sc.evBytes);   // 16-byte records in, 2-byte event codes out
+  if (rw.R == 0) return;
+  const uint32_t R = rw.R;
+  BANI_SCRATCH(bani_mapping, rows, R);
+  rw.rows = rows; rw.frag.alloc(R, st);
+  { Stage sg(ctx, "report", 44.0 * R);
+    rows_kernel<<<nblk(C), 256, 0, st>>>(ra, keep.p, keepScan.p, rows.p, rw.frag.p); ctx->launches++; }
+  if (hostRows) {
+    size_t old = hostRows->size(); hostRows->resize(old + R);
+    BANI_CUDA(cudaMemcpyAsync(hostRows->data() + old, rows.p, sizeof(bani_mapping) * (size_t)R, cudaMemcpyDeviceToHost, st));
+    BANI_CUDA(cudaStreamSynchronize(st));
+  }
+}
+
+// Stages C..H of one piece.  Returns P_PIECE_MAPPED, or the reason to map the piece in halves instead; the piece's
+// counters and results reach `out` (query slots mapped to query ids) only when it is mapped.
+static PathId map_piece(Ctx *ctx, const Index *ix, const QSketch &qs, const QPiece &pc, CgiState *cgi, bool wantRows, MapOutput &out)
+{
+  bani_map_counters ctr{};
+  uint64_t pp[NPATH] = {};
+  CgiResult res;
+  ctx->mark("piece: begin");
+  if (pc.F > 0 && ix->M > 0) {
+    ctx->upload_lut(pc.smax, pc.sCount.p, pc.F);
+    if (pc.T > 0 && pc.smax > 0) {
+      Hits h; Cands cd; Scores sc; Rows rw;
+      lookup(ctx, ix, pc, pp, h);
+      const unsigned long long maxHits = (unsigned long long)std::max(1ll, ctx->flags.maxHitsPerPiece);    // 1.6 G hits per pass by default
+      if (h.N > maxHits && pc.nq > 1) return P_PIECE_SPLIT_HITS;                      // too many hits for one pass
+      if (h.N > 0xfffffff0ull) fail(BANI_ERR_LIMIT, "one query genome gathers more than 2^32 index hits");
+      ctr.hits = h.N;
+      if (h.N > 0) l1_candidates(ctx, ix, pc, h, pp, cd);
+      ctr.candidates = cd.C;
+      if (cd.C > 0) {
+        if (l2_candidates(ctx, ix, pc, cd, pp, sc) == P_PIECE_SPLIT_EVENTS) return P_PIECE_SPLIT_EVENTS;
+        report(ctx, pc, cd, sc, ctr, wantRows ? &out.rows : nullptr, rw);
+      }
+      // H: the identity reduction (cgi.cu)
+      if (rw.R > 0 && cgi) cgi_piece(ctx, *cgi, rw.rows.p, rw.frag.p, rw.R, pc.fragQuery.p, pc.nq, pp, res);
+    }
+    ctr.sum_s = pc.T;
+  }
+  ctr.fragments = pc.F;
+  out.ctr.hits += ctr.hits; out.ctr.candidates += ctr.candidates; out.ctr.n2 += ctr.n2; out.ctr.mappings += ctr.mappings;
+  out.ctr.fragments += ctr.fragments; out.ctr.sum_s += ctr.sum_s;
+  if (ctx->flags.countPaths) {
+    pp[P_PIECE_MAPPED]++;
+    for (int i = 0; i < NPATH; i++) ctx->paths[i] += pp[i];
+  }
+  const int32_t *queryId = qs.queryId.data() + pc.q0;
+  const uint64_t *totalFragments = qs.totalFragments.data() + pc.q0;
+  if (!res.count.empty()) append_cgi_rows(res.count.data(), res.ident.data(), pc.nq, ix->nGenomes, queryId, totalFragments, out.cgi);
+  for (bani_cgi_result r : res.pairs) {
+    if (r.countSeq <= 0) continue;
+    const int slot = r.qryGenomeId;
+    r.qryGenomeId = queryId[slot]; r.totalQueryFragments = (int32_t)totalFragments[slot];
+    out.cgi.push_back(r);
+  }
+  for (bani_frag_mapping &m : res.frags) m.qryGenomeId = queryId[m.qryGenomeId];
+  out.frags.insert(out.frags.end(), res.frags.begin(), res.frags.end());
+  return P_PIECE_MAPPED;
+}
+
 void qsketch_map(Ctx *ctx, const Index *ix, const QSketch *const *sketches, int32_t nSketches,
                  bool wantRows, bool wantCgi, MapOutput &out, bool wantFrags)
 {
   cudaStream_t st = ctx->stream;
   wantCgi = wantCgi || wantFrags;
   const int k = ctx->prm.kmer_size, w = ctx->prm.window_size, fragLen = ctx->prm.frag_len;
-  const float pid = ctx->prm.perc_identity;
   if (ix->device != ctx->device) fail(BANI_ERR_ARG, "index lives on another device");
   if (ix->k != k || ix->w != w || ix->fragLen != fragLen)
     fail(BANI_ERR_ARG, "index was built with other parameters (k %d w %d fragLen %d)", ix->k, ix->w, ix->fragLen);
   if (wantCgi && fragLen <= 20) fail(BANI_ERR_ARG, "fragment length must exceed 20 for the identity reduction");
-  const int cmw = fragLen - (w - 1) - (k - 1);         // computeMap.hpp:427
   out.ctr = bani_map_counters{};
-  const int nG = ix->nGenomes;
-
-  // the 2-way table holds a bounded number of queries at a time (4-byte bins, 8-byte keys in the fragment-row mode)
-  uint64_t qMaxByTable = 1u << 30;
-  const uint64_t binBytes = wantFrags ? 8 : 4;
-  if (wantCgi && ix->totalBins) qMaxByTable = std::max<uint64_t>(1, ((uint64_t)3 << 30) / (binBytes * ix->totalBins));
-  if (ctx->flags.cgiTableQueries > 0) qMaxByTable = std::min<uint64_t>(qMaxByTable, (uint64_t)ctx->flags.cgiTableQueries);
-  // a piece whose L2 event streams would take more is mapped in halves
-  const double evLimit = ctx->flags.eventBytesPerPiece > 0 ? (double)ctx->flags.eventBytesPerPiece : 0.25 * (double)ctx->memTotal;
-  const bool countPaths = ctx->flags.countPaths != 0;
-
-  DevBuf<uint32_t> table; DevBuf<unsigned long long> table64; DevBuf<uint8_t> touched; DevBuf<int32_t> d_gce;
-  uint64_t tableQ = 0;
-  if (wantCgi) {
-    d_gce.alloc(std::max(nG, 1), st);
-    if (nG) BANI_CUDA(cudaMemcpyAsync(d_gce.p, ix->seqsByFile.data(), 4 * (size_t)nG, cudaMemcpyHostToDevice, st));
-  }
+  std::unique_ptr<CgiState> cgi;
+  if (wantCgi) cgi = std::make_unique<CgiState>(ctx, ix, wantFrags);
 
   for (int32_t si = 0; si < nSketches; si++) {
-   const QSketch *qs = sketches[si];
-   if (!qs) fail(BANI_ERR_ARG, "null query sketch");
-   if (qs->device != ctx->device) fail(BANI_ERR_ARG, "query sketch lives on another device");
-   if (qs->k != k || qs->w != w || qs->fragLen != fragLen) fail(BANI_ERR_ARG, "query sketch was built with other parameters");
-   const unsigned long long maxHits = (unsigned long long)std::max(1ll, ctx->flags.maxHitsPerPiece);           // 1.6 G hits per pass by default
-   std::deque<const QPiece *> work;
-   std::vector<std::unique_ptr<QPiece>> slices;
-   for (const auto &pcp : qs->pieces) work.push_back(pcp.get());
-   while (!work.empty()) {
-    const QPiece &pc = *work.front();
-    work.pop_front();
-    const int nQc = pc.nq, q0 = pc.q0;
-    const int32_t F = pc.F;
-    const uint64_t T = pc.T;
-    const int smax = pc.smax;
-    bool split = false;
-    uint64_t pp[NPATH] = {};                 // path counters of this piece, kept if it is not split
-    // halve the piece at a query boundary (by fragments) and do the halves instead
-    auto split_in_halves = [&](PathId why) {
-      if (countPaths) ctx->paths[why]++;
-      int qm = 1;
-      while (qm < nQc - 1 && pc.qFragOff[qm] < F / 2) qm++;
-      slices.push_back(slice_piece(ctx, pc, qm, nQc)); work.push_front(slices.back().get());
-      slices.push_back(slice_piece(ctx, pc, 0, qm)); work.push_front(slices.back().get());
-      split = true;
-    };
-    View<uint32_t> fragHash; fragHash.p = pc.fragHash.p; fragHash.n = T;
-    View<uint32_t> segStart; segStart.p = pc.segStart.p; segStart.n = (size_t)F + 1;
-    View<int32_t> sCount; sCount.p = pc.sCount.p; sCount.n = F;
-    View<int32_t> d_fragQuery; d_fragQuery.p = pc.fragQuery.p; d_fragQuery.n = F;
-    View<int32_t> d_fragSeqId; d_fragSeqId.p = pc.fragSeqId.p; d_fragSeqId.n = F;
-
-    std::vector<int32_t> hCount; std::vector<float> hIdent;      // dense stage H: allocated once the piece has rows to reduce
-    std::vector<bani_cgi_result> hPairs;                        // sparse stage H: (query slot, genome) rows
-    std::vector<bani_frag_mapping> hFrags;
-
-    ctx->mark("piece: begin");
-    if (F > 0 && ix->M > 0) {
-      ctx->upload_lut(smax, pc.sCount.p, F);
-
-      if (T > 0 && smax > 0) {
-        // ---- C: lookup
-        BANI_SCRATCH(uint32_t, hitLo, T + 1);
-        BANI_SCRATCH(uint32_t, hitCnt, T + 1);
-        BANI_SCRATCH(unsigned long long, hitOff, T + 1);
-        DevBuf<unsigned long long> walkCtr;
-        if (countPaths) { walkCtr.alloc(2, st); BANI_CUDA(cudaMemsetAsync(walkCtr.p, 0, 16, st)); }
-        { Stage sg(ctx, "lookup", 12.0 * T);
-          // the membership filter pays when most probes miss: not for queries that are genomes of this very index
-          const bool useFilt = ix->filt.p && pc.memberOf != ix->uid;
-          lookup_kernel<<<nblk(T + 1), 256, 0, st>>>(fragHash.p, (uint32_t)T, ix->tab.p, (1u << ix->tabBits) - 1u, ix->ukeys.p, ix->uoff.p,
-                                                   ix->dir.p, ix->dirBits, useFilt ? ix->filt.p : nullptr,
-                                                   useFilt ? (uint32_t)((1ull << ix->filtBits) - 1ull) : 0u, hitLo.p, hitCnt.p, walkCtr.p);
-          ctx->launches++;
-          size_t tb = cub_scan_u64_temp(T + 1);
-          BANI_SCRATCH(uint8_t, tmp, tb);
-          cub_exclusive_sum_u32_to_u64(tmp.p, tb, hitCnt.p, (uint64_t *)hitOff.p, T + 1, st); }
-        unsigned long long N = 0;
-        BANI_CUDA(cudaMemcpyAsync(&N, hitOff.p + T, 8, cudaMemcpyDeviceToHost, st));
-        if (countPaths) BANI_CUDA(cudaMemcpyAsync(pp + P_LOOKUP_WALK_SATURATED, walkCtr.p, 16, cudaMemcpyDeviceToHost, st));
-        BANI_CUDA(cudaStreamSynchronize(st));
-        ctx->mark("piece: lookup done");
-        if (N > maxHits && nQc > 1) split_in_halves(P_PIECE_SPLIT_HITS);          // too many hits for one pass
-        if (!split && N > 0xfffffff0ull) fail(BANI_ERR_LIMIT, "one query genome gathers more than 2^32 index hits");
-        if (!split) out.ctr.hits += N;
-
-        if (N > 0 && !split) {
-          // ---- D+E: hits -> L1 candidate regions.  Fragments with at most FRAG_L1_MAX hits are handled by
-          //      one CTA each (hits.cu); the others go through the device-wide sort below.  Both write their
-          //      regions to a staging area addressed by the fragment's hit offset; a scan + copy makes them dense.
-          BANI_SCRATCH(uint32_t, candCount, (size_t)F + 1);
-          BANI_SCRATCH(uint32_t, candOff, (size_t)F + 1);
-          BANI_SCRATCH(uint32_t, fragClass, F);
-          BANI_SCRATCH(uint32_t, classList, (size_t)FRAG_NCLASS * F);
-          BANI_SCRATCH(uint32_t, classCount, FRAG_NCLASS + 2);
-          BANI_SCRATCH(int32_t, stSeq, N);
-          BANI_SCRATCH(int32_t, stStart, N);
-          BANI_SCRATCH(int32_t, stEnd, N);
-          const long long maxFast = std::max(0ll, std::min(ctx->flags.fragL1Max, (long long)FRAG_L1_MAX));
-          uint32_t hClass[FRAG_NCLASS + 2];
-          { Stage sg(ctx, "frag_l1", 12.0 * N);                // 4 B list entry + 8 B (seqId, wpos) per hit
-            frag_classify(ctx, segStart.p, hitOff.p, F, candCount.p, fragClass.p, classCount.p, classList.p, (unsigned long long)maxFast);
-            BANI_CUDA(cudaMemcpyAsync(hClass, classCount.p, sizeof hClass, cudaMemcpyDeviceToHost, st));
-            BANI_CUDA(cudaStreamSynchronize(st));
-            for (int i = 0; i <= FRAG_NCLASS; i++) pp[P_L1_CLASS0 + i] += hClass[i];
-            FragL1Args fa; fa.segStart = segStart.p; fa.sCount = sCount.p; fa.F = F; fa.hitLo = hitLo.p; fa.hitCnt = hitCnt.p; fa.hitOff = hitOff.p;
-            fa.posIdx = ix->posIdx.p; fa.recPos = ix->pos8.p; fa.minHits = ctx->d_minHits.p; fa.fragLen = fragLen;
-            fa.keyBits = 1; while (fa.keyBits < 32 && (1ull << fa.keyBits) < ix->M) fa.keyBits++;
-            fa.stSeq = stSeq.p; fa.stStart = stStart.p; fa.stEnd = stEnd.p; fa.candCount = candCount.p;
-            frag_l1_fast(ctx, fa, classList.p, hClass); }
-          if (hClass[FRAG_NCLASS] > 0) {
-            // ---- device-wide path for the oversized fragments: (fragment, record) keys, one radix sort, flags + scan + write
-            BANI_SCRATCH(uint32_t, bigCnt, T + 1);
-            BANI_SCRATCH(unsigned long long, bigOff, T + 1);
-            mask_hits_kernel<<<nblk(T + 1), 256, 0, st>>>(segStart.p, F, (uint32_t)T, hitCnt.p, fragClass.p, bigCnt.p); ctx->launches++;
-            { size_t tb = cub_scan_u64_temp(T + 1);
-              BANI_SCRATCH(uint8_t, tmp, tb);
-              cub_exclusive_sum_u32_to_u64(tmp.p, tb, bigCnt.p, (uint64_t *)bigOff.p, T + 1, st); }
-            unsigned long long NB = 0;
-            BANI_CUDA(cudaMemcpyAsync(&NB, bigOff.p + T, 8, cudaMemcpyDeviceToHost, st));
-            BANI_CUDA(cudaStreamSynchronize(st));
-            BANI_SCRATCH(unsigned long long, keysA, NB);
-            BANI_SCRATCH(unsigned long long, keysB, NB);
-            { Stage sg(ctx, "hit_gather", 12.0 * NB);
-              gather_kernel<<<nblk(T), 256, 0, st>>>(segStart.p, F, (uint32_t)T, hitLo.p, bigCnt.p, bigOff.p, ix->posIdx.p, keysA.p); ctx->launches++; }
-            int fbits = 1; while ((1ll << fbits) < F) fbits++;
-            { Stage sg(ctx, "hit_sort", 16.0 * NB);
-              size_t tb = cub_sort_keys_u64_temp(NB);
-              BANI_SCRATCH(uint8_t, tmp, tb);
-              cub_sort_keys_u64(tmp.p, tb, (const uint64_t *)keysA.p, (uint64_t *)keysB.p, NB, 0, 32 + fbits, st); }
-            L1Args la; la.keys = keysB.p; la.N = NB; la.segStart = segStart.p; la.hitOff = bigOff.p; la.sCount = sCount.p;
-            la.minHits = ctx->d_minHits.p; la.recSeq = ix->seqId.p; la.recWpos = ix->wpos.p; la.fragLen = fragLen;
-            BANI_SCRATCH(uint32_t, head, NB + 1);
-            BANI_SCRATCH(uint32_t, headScan, NB + 1);
-            { Stage sg(ctx, "l1_flags", 8.0 * NB);
-              l1_flag_kernel<<<nblk(NB + 1), 256, 0, st>>>(la, head.p);
-              ctx->launches++;
-              size_t tb = cub_scan_u32_temp(NB + 1);
-              BANI_SCRATCH(uint8_t, tmp, tb);
-              cub_exclusive_sum_u32(tmp.p, tb, head.p, headScan.p, NB + 1, st); }
-            uint32_t CB = 0;
-            BANI_CUDA(cudaMemcpyAsync(&CB, headScan.p + NB, 4, cudaMemcpyDeviceToHost, st));
-            BANI_CUDA(cudaStreamSynchronize(st));
-            if (CB > 0) {
-              BANI_SCRATCH(int32_t, bFrag, CB);
-              BANI_SCRATCH(int32_t, bSeq, CB);
-              BANI_SCRATCH(int32_t, bStart, CB);
-              BANI_SCRATCH(int32_t, bEnd, CB);
-              Stage sg(ctx, "l1_write", 8.0 * NB);
-              l1_write_kernel<<<nblk(NB), 256, 0, st>>>(la, head.p, headScan.p, bFrag.p, bSeq.p, bStart.p, bEnd.p); ctx->launches++;
-              cand_stage(ctx, bFrag.p, bSeq.p, bStart.p, bEnd.p, CB, segStart.p, hitOff.p, stSeq.p, stStart.p, stEnd.p, candCount.p);
-            }
-          }
-          { size_t tb = cub_scan_u32_temp((size_t)F + 1);
-            BANI_SCRATCH(uint8_t, tmp, tb);
-            BANI_CUDA(cudaMemsetAsync(candCount.p + F, 0, 4, st));
-            cub_exclusive_sum_u32(tmp.p, tb, candCount.p, candOff.p, (size_t)F + 1, st); }
-          uint32_t C = 0;
-          BANI_CUDA(cudaMemcpyAsync(&C, candOff.p + F, 4, cudaMemcpyDeviceToHost, st));
-          BANI_CUDA(cudaStreamSynchronize(st));
-          out.ctr.candidates += C;
-
-          if (C > 0) {
-            BANI_SCRATCH(int32_t, cFrag, C);
-            BANI_SCRATCH(int32_t, cSeq, C);
-            BANI_SCRATCH(int32_t, cStart, C);
-            BANI_SCRATCH(int32_t, cEnd, C);
-            BANI_SCRATCH(int32_t, cPos, C);
-            BANI_SCRATCH(int32_t, cBest, C);
-            cand_compact(ctx, segStart.p, hitOff.p, F, candCount.p, candOff.p, stSeq.p, stStart.p, stEnd.p, cFrag.p, cSeq.p, cStart.p, cEnd.p);
-
-            // ---- F: L2
-            L2Args l2; l2.cFrag = cFrag.p; l2.cSeq = cSeq.p; l2.cStart = cStart.p; l2.cEnd = cEnd.p; l2.C = C;
-            l2.fragHash = fragHash.p; l2.segStart = segStart.p; l2.sCount = sCount.p;
-            l2.recHash = ix->hash.p; l2.recWpos = ix->wpos.p; l2.recLink = ix->link.p; l2.contigRecOff = ix->contigRecOff.p;
-            l2.fragLen = fragLen; l2.cmw = cmw; l2.smax = smax;
-            l2.stride = ((size_t)2 * (smax + 2) + smax + 15) / 16 * 16;
-            const unsigned blocks = (unsigned)std::min<uint64_t>((C + 63) / 64, (uint64_t)ctx->smCount * 16);
-            BANI_SCRATCH(uint8_t, scratch, (size_t)blocks * 64 * l2.stride);
-            BANI_SCRATCH(unsigned long long, d_n2, 1);
-            BANI_CUDA(cudaMemsetAsync(d_n2.p, 0, 8, st));
-            l2.scratch = scratch.p; l2.cPos = cPos.p; l2.cBest = cBest.p; l2.onlyFlagged = 1;
-            size_t idEv = (size_t)-1; double evBytes = 0;
-            {
-              unsigned long long totalSteps = 0;
-              Stage sgb(ctx, "l2_bounds", 12.0 * C);
-              BANI_SCRATCH(uint32_t, fragCandOff, (size_t)F + 1);
-              frag_cand_off_kernel<<<nblk((uint64_t)F + 1), 256, 0, st>>>(cFrag.p, C, F, fragCandOff.p);
-              ctx->launches++;
-              L2PArgs lp; lp.cFrag = cFrag.p; lp.cSeq = cSeq.p; lp.cStart = cStart.p; lp.cEnd = cEnd.p; lp.C = C;
-              lp.fragCandOff = fragCandOff.p; lp.fragHash = fragHash.p; lp.segStart = segStart.p; lp.sCount = sCount.p;
-              lp.rec = ix->rec.p; lp.recWposSoA = ix->wpos.p; lp.contigRecOff = ix->contigRecOff.p; lp.fragLen = fragLen; lp.cmw = cmw;
-              lp.rec8 = ix->rec8.p; lp.recLink = ix->link.p; lp.blkMax = ix->blkMax.p; lp.stage = ctx->flags.l2Stage;
-              // fast path: needs the window links of the index (cmw >= 2) and ranks that fit the event code
-              // (and whose per-warp state fits the shared-memory budget of l2_seq_kernel: larger sketches take l2_kernel)
-              // (the switch l2_fast = 0 sends every candidate to l2_kernel)
-              lp.sLimit = (ctx->flags.l2Fast && cmw >= 2 && ix->cmw == cmw && ix->rec8.p) ? std::min(std::min(smax, L2_SMAX), L2_SHM_BUDGET / (L2S_WARPS * 32) - 2) : 0;
-              // bucket width near 0 ~ 2^32 / (s * w): minimizer hashes are minima of w hashes, density w/2^32 at 0
-              lp.nBuckets = ((uint64_t)C >= 8ull * (uint64_t)F) ? L2E_BUCKETS : 1024;      // few candidates per fragment: building a big directory is not worth it
-              { const int forced = ctx->flags.l2eBuckets;
-                if (forced == 1024 || forced == L2E_BUCKETS) lp.nBuckets = forced; }
-              { int sh = lp.nBuckets == L2E_BUCKETS ? 20 : 22; while (sh > 8 && ((uint64_t)std::max(smax, 1) * (uint64_t)w << sh) > ((1ull << 32) * (uint64_t)(L2E_BUCKETS / lp.nBuckets))) sh--; lp.shiftA = sh; }
-              lp.warpBytes = (uint32_t)(std::max(lp.sLimit, 1) + 1) * 32u;      // one state byte per rank 0..s and lane
-              BANI_SCRATCH(uint32_t, cB0, C);          // (one scratch slot per source line)
-              BANI_SCRATCH(uint32_t, cE0, C);
-              BANI_SCRATCH(uint32_t, cLast, C);
-              BANI_SCRATCH(uint32_t, cNEv, C);
-              BANI_SCRATCH(uint32_t, cChunks, (size_t)C + 1);
-              BANI_SCRATCH(uint32_t, cOff, (size_t)C + 1);
-              BANI_SCRATCH(uint16_t, cMB, (size_t)C + 1);
-              lp.cMB = cMB.p;
-              lp.cB0 = cB0.p; lp.cE0 = cE0.p; lp.cLast = cLast.p; lp.cNEv = cNEv.p; lp.cChunks = cChunks.p; lp.cOff = cOff.p;
-              lp.cPos = cPos.p; lp.cBest = cBest.p; lp.ctr_n2 = d_n2.p; lp.events = nullptr; lp.perm = nullptr;
-              l2_bounds_kernel<<<nblk((uint64_t)C + 1), 256, 0, st>>>(lp); ctx->launches++;
-              if (countPaths) pp[P_L2_EXACT_AT_BOUNDS] += count_exact(ctx, cBest.p, C);
-              if (lp.sLimit > 0) {
-                // candidates by descending event count: rank g -> warp g / 32, lane g % 32 of the sequential kernel
-                BANI_SCRATCH(uint32_t, skey, C);
-                BANI_SCRATCH(uint32_t, skey2, C);
-                BANI_SCRATCH(uint32_t, sval, C);
-                BANI_SCRATCH(uint32_t, perm, C);
-                l2_sortkey_kernel<<<nblk(C), 256, 0, st>>>(cNEv.p, C, skey.p, sval.p); ctx->launches++;
-                { size_t tb = cub_sort_pairs_u32_temp(C);
-                  BANI_SCRATCH(uint8_t, tmp, tb);
-                  cub_sort_pairs_u32(tmp.p, tb, skey.p, skey2.p, sval.p, perm.p, C, 20, st); }
-                lp.perm = perm.p;
-                // event streams, interleaved per warp: step k of lane l of warp G is the 32-byte slot (grpOff[G] + k) * 32 + l,
-                // so a warp reads 1 KB contiguous per step while every 32-byte sector still belongs to one candidate
-                const uint32_t nGrp = (C + 31) / 32;
-                BANI_SCRATCH(uint32_t, grpSteps, (size_t)nGrp + 1);
-                BANI_SCRATCH(unsigned long long, grpOff, (size_t)nGrp + 1);
-                l2_group_steps_kernel<<<nblk((uint64_t)nGrp + 1), 256, 0, st>>>(cChunks.p, perm.p, C, nGrp, grpSteps.p); ctx->launches++;
-                { size_t tb = cub_scan_u64_temp((size_t)nGrp + 1);
-                  BANI_SCRATCH(uint8_t, tmp, tb);
-                  cub_exclusive_sum_u32_to_u64(tmp.p, tb, grpSteps.p, (uint64_t *)grpOff.p, (size_t)nGrp + 1, st); }
-                unsigned long long totalGrpSteps = 0;
-                BANI_CUDA(cudaMemcpyAsync(&totalGrpSteps, grpOff.p + nGrp, 8, cudaMemcpyDeviceToHost, st));
-                BANI_CUDA(cudaStreamSynchronize(st));
-                totalSteps = totalGrpSteps * 32;                      // 32-byte slots
-                if ((double)totalSteps * 32.0 > evLimit && nQc > 1) {
-                  // the event streams of this piece would take more than a quarter of the device (small windows make many
-                  // events per hit): map its halves instead, so that they fit beside the index
-                  out.ctr.hits -= N; out.ctr.candidates -= C;
-                  split_in_halves(P_PIECE_SPLIT_EVENTS);
-                  goto piece_done;
-                }
-                if (totalSteps > 0xfffffff0ull) fail(BANI_ERR_LIMIT, "query chunk schedules more than 2^36 window events");
-                BANI_SCRATCH(uint16_t, events, (size_t)totalSteps * 16 + 64);
-                lp.events = events.p; lp.grpOff = grpOff.p;
-                l2_stream_base_kernel<<<nblk(C), 256, 0, st>>>(perm.p, grpOff.p, C, cOff.p); ctx->launches++;
-                // CTA size of the events kernel by candidates per fragment (warp per candidate: no idle warps in small shards)
-                const int evNT = ((uint64_t)C >= 6ull * (uint64_t)F) ? 256 : ((uint64_t)C >= 3ull * (uint64_t)F) ? 128 : 64;
-                if (countPaths) {
-                  // candidates with window events, by the variant of l2_events_kernel that writes them
-                  std::vector<uint32_t> nEv(C); std::vector<uint16_t> mb(C);
-                  BANI_CUDA(cudaMemcpyAsync(nEv.data(), cNEv.p, 4 * (size_t)C, cudaMemcpyDeviceToHost, st));
-                  BANI_CUDA(cudaMemcpyAsync(mb.data(), cMB.p, 2 * (size_t)C, cudaMemcpyDeviceToHost, st));
-                  BANI_CUDA(cudaStreamSynchronize(st));
-                  uint64_t withEv = 0, staged = 0;
-                  for (uint32_t c = 0; c < C; c++) if (nEv[c]) { withEv++; staged += mb[c] != 0xFFFFu; }
-                  pp[evNT == 256 ? P_L2_EVENTS_NT256 : evNT == 128 ? P_L2_EVENTS_NT128 : P_L2_EVENTS_NT64] += withEv;
-                  pp[lp.nBuckets == L2E_BUCKETS ? P_L2_DIR4096 : P_L2_DIR1024] += withEv;
-                  pp[P_L2_STAGED] += staged; pp[P_L2_DIRECT] += withEv - staged;
-                }
-                const size_t shmE = 4 * ((size_t)(evNT / 32) * (L2E_RING / 2) + (size_t)lp.sLimit + 4 + L2E_BUCKETS + 4 + 2) + 8 * ((size_t)lp.sLimit + 4) + 16;
-                const size_t shmS = (size_t)L2S_WARPS * lp.warpBytes;
-                if (shmE > (size_t)L2_SHM_BUDGET || shmS > (size_t)L2_SHM_BUDGET) fail(BANI_ERR_INTERNAL, "L2 shared-memory budget exceeded");
-                if (ctx->first_time((const void *)l2_seq_kernel)) {
-                  BANI_CUDA(cudaFuncSetAttribute(l2_events_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, L2_SHM_BUDGET));
-                  BANI_CUDA(cudaFuncSetAttribute(l2_events_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, L2_SHM_BUDGET));
-                  BANI_CUDA(cudaFuncSetAttribute(l2_events_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, L2_SHM_BUDGET));
-                  BANI_CUDA(cudaFuncSetAttribute(l2_seq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, L2_SHM_BUDGET));
-                  BANI_CUDA(cudaFuncSetAttribute(l2_seq_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
-                }
-                sgb.stop();
-                { Stage sg(ctx, "l2_events"); idEv = sg.id(); evBytes = 32.0 * (double)totalSteps;
-                  if (evNT == 256) l2_events_kernel<256><<<F, 256, shmE, st>>>(lp);
-                  else if (evNT == 128) l2_events_kernel<128><<<F, 128, shmE, st>>>(lp);
-                  else l2_events_kernel<64><<<F, 64, shmE, st>>>(lp);
-                  ctx->launches++; }
-                { Stage sg(ctx, "l2_seq", evBytes + 16.0 * C);       // the event codes in, {position, shared} out
-                  l2_seq_kernel<<<nblk(C, L2S_WARPS * 32), L2S_WARPS * 32, shmS, st>>>(lp); ctx->launches++; }
-              }
-              sgb.stop();
-              if (countPaths) pp[P_L2_EXACT_TOTAL] += count_exact(ctx, cBest.p, C);
-              // exact slow path for whatever the fast path flagged (counter overflow, very large sketches)
-              Stage sgs(ctx, "l2_exact");
-              l2_kernel<<<blocks, 64, 0, st>>>(l2); ctx->launches++;
-            }
-
-            // ---- G: report
-            RepArgs ra; ra.cFrag = cFrag.p; ra.cSeq = cSeq.p; ra.cPos = cPos.p; ra.cBest = cBest.p; ra.C = C;
-            ra.sCount = sCount.p; ra.fragSeqId = d_fragSeqId.p; ra.rowOff = ctx->d_rowOff.p; ra.ident = ctx->d_ident.p;
-            ra.upper = ctx->d_upper.p; ra.pid = pid; ra.fragLen = fragLen;
-            BANI_SCRATCH(uint32_t, keep, C + 1);
-            BANI_SCRATCH(uint32_t, keepScan, C + 1);
-            keep_flag_kernel<<<nblk(C + 1), 256, 0, st>>>(ra, keep.p);
-            ctx->launches++;
-            { size_t tb = cub_scan_u32_temp(C + 1);
-            BANI_SCRATCH(uint8_t, tmp, tb);
-              cub_exclusive_sum_u32(tmp.p, tb, keep.p, keepScan.p, C + 1, st); }
-            uint32_t R = 0; unsigned long long n2 = 0;
-            BANI_CUDA(cudaMemcpyAsync(&R, keepScan.p + C, 4, cudaMemcpyDeviceToHost, st));
-            BANI_CUDA(cudaMemcpyAsync(&n2, d_n2.p, 8, cudaMemcpyDeviceToHost, st));
-            BANI_CUDA(cudaStreamSynchronize(st));
-            out.ctr.n2 += n2; out.ctr.mappings += R;
-            ctx->mark("piece: L1 + L2 done");
-            Stage::set_bytes(ctx, idEv, 16.0 * (double)n2 + evBytes);   // 16-byte records in, 2-byte event codes out
-            if (R > 0) {
-              BANI_SCRATCH(bani_mapping, rows, R);
-              DevBuf<int32_t> rFrag(R, st);
-              { Stage sg(ctx, "report", 44.0 * R);
-                rows_kernel<<<nblk(C), 256, 0, st>>>(ra, keep.p, keepScan.p, rows.p, rFrag.p); ctx->launches++; }
-              if (wantRows) {
-                size_t old = out.rows.size(); out.rows.resize(old + R);
-                BANI_CUDA(cudaMemcpyAsync(out.rows.data() + old, rows.p, sizeof(bani_mapping) * (size_t)R, cudaMemcpyDeviceToHost, st));
-                BANI_CUDA(cudaStreamSynchronize(st));
-              }
-              // ---- H: CGI.  Sparse when the dense (query, genome) output of the piece would exceed both its rows and 2^22
-              // entries (many small genomes; DESIGN.md section 6), unless the cgi_sparse switch forces a path
-              const bool sparse = wantCgi && (ctx->flags.cgiSparse >= 0 ? ctx->flags.cgiSparse == 1
-                                                                        : (uint64_t)nQc * nG > std::max<uint64_t>(R, CGI_SPARSE_MIN_PAIRS));
-              if (sparse) {
-                int qBits = 0; while ((1ull << qBits) <= (uint64_t)nQc) qBits++;                 // slots 0 .. nQc (the sentinel)
-                int binBits = 1; while ((1ull << binBits) < ix->totalBins) binBits++;
-                if (qBits + binBits > 64) fail(BANI_ERR_LIMIT, "sparse identity reduction: %d query bits + %d bin bits exceed 64", qBits, binBits);
-                CgiArgs ca; ca.rows = rows.p; ca.rFrag = rFrag.p; ca.R = R; ca.fragQuery = d_fragQuery.p;
-                ca.contigGenome = ix->contigGenome.p; ca.contigBinOff = ix->contigBinOff.p; ca.fragLen = fragLen;
-                ca.totalBins = ix->totalBins; ca.nGenomes = nG; ca.table = nullptr; ca.touched = nullptr; ca.qLo = 0; ca.qHi = nQc;
-                BANI_SCRATCH(unsigned long long, spKey, R);
-                BANI_SCRATCH(unsigned long long, spKeySorted, R);
-                BANI_SCRATCH(uint32_t, spRow, R);
-                BANI_SCRATCH(uint32_t, spRowSorted, R);
-                BANI_SCRATCH(uint32_t, binHead, (size_t)R + 1);
-                BANI_SCRATCH(uint32_t, binIdx, (size_t)R + 1);
-                BANI_SCRATCH(unsigned long long, binKey, R);
-                BANI_SCRATCH(uint32_t, binRow, R);
-                BANI_SCRATCH(uint32_t, pairHead, (size_t)R + 1);
-                BANI_SCRATCH(uint32_t, pairIdx, (size_t)R + 1);
-                BANI_SCRATCH(bani_cgi_result, dPairs, R);
-                Stage sg(ctx, "cgi_sparse", 150.0 * R);
-                pp[P_CGI_SPARSE]++;
-                cgi_sparse_key_kernel<<<nblk(R), 256, 0, st>>>(ca, binBits, nQc, spKey.p, spRow.p);
-                ctx->launches++;
-                { size_t tb = cub_sort_pairs_u64_u32_temp(R);
-                  BANI_SCRATCH(uint8_t, tmp, tb);
-                  cub_sort_pairs_u64_u32(tmp.p, tb, (const uint64_t *)spKey.p, (uint64_t *)spKeySorted.p, spRow.p, spRowSorted.p, R, qBits + binBits, st); }
-                cgi_sparse_bin_head_kernel<<<nblk((uint64_t)R + 1), 256, 0, st>>>(spKeySorted.p, R, (unsigned long long)nQc << binBits, binHead.p);
-                ctx->launches++;
-                const size_t tbScan = cub_scan_u32_temp((size_t)R + 1);
-                BANI_SCRATCH(uint8_t, scanTmp, tbScan);
-                cub_exclusive_sum_u32(scanTmp.p, tbScan, binHead.p, binIdx.p, (size_t)R + 1, st);
-                BANI_CUDA(cudaMemsetAsync(pairHead.p, 0, 4 * ((size_t)R + 1), st));
-                cgi_sparse_bin_max_kernel<<<nblk(R), 256, 0, st>>>(ca, spKeySorted.p, spRowSorted.p, R, binBits, binHead.p, binIdx.p,
-                                                                   binKey.p, binRow.p, pairHead.p);
-                ctx->launches++;
-                cub_exclusive_sum_u32(scanTmp.p, tbScan, pairHead.p, pairIdx.p, (size_t)R + 1, st);
-                cgi_sparse_pair_kernel<<<nblk(R), 256, 0, st>>>(ca, binKey.p, binRow.p, binIdx.p + R, pairHead.p, pairIdx.p, wantFrags, dPairs.p);
-                ctx->launches++;
-                uint32_t nBins = 0, nPairs = 0;
-                BANI_CUDA(cudaMemcpyAsync(&nBins, binIdx.p + R, 4, cudaMemcpyDeviceToHost, st));
-                BANI_CUDA(cudaMemcpyAsync(&nPairs, pairIdx.p + R, 4, cudaMemcpyDeviceToHost, st));
-                BANI_CUDA(cudaStreamSynchronize(st));
-                // the bin winners are already in (query slot, global bin) order: the fragment rows need no second sort
-                if (wantFrags && nBins > 0) {
-                  BANI_SCRATCH(bani_frag_mapping, dFrags, nBins);
-                  cgi_frag_gather_kernel<<<nblk(nBins), 256, 0, st>>>(rows.p, binKey.p, binRow.p, nBins, dFrags.p);
-                  ctx->launches++;
-                  hFrags.resize(nBins);
-                  BANI_CUDA(cudaMemcpyAsync(hFrags.data(), dFrags.p, sizeof(bani_frag_mapping) * (size_t)nBins, cudaMemcpyDeviceToHost, st));
-                }
-                hPairs.resize(nPairs);
-                if (nPairs) BANI_CUDA(cudaMemcpyAsync(hPairs.data(), dPairs.p, sizeof(bani_cgi_result) * (size_t)nPairs, cudaMemcpyDeviceToHost, st));
-                BANI_CUDA(cudaStreamSynchronize(st));
-                ctx->mark("piece: sparse identity rows on host");
-              } else if (wantCgi) {
-                // ---- H: CGI, at most tableQ queries of the piece per pass over the rows
-                hCount.assign((size_t)nQc * nG, 0); hIdent.assign((size_t)nQc * nG, 0.f);
-                const uint64_t needQ = std::min<uint64_t>(qMaxByTable, std::max<uint64_t>(nQc, 1));
-                if (needQ > tableQ) {
-                  tableQ = needQ;
-                  if (wantFrags) table64.alloc((size_t)tableQ * ix->totalBins, st);
-                  else table.alloc((size_t)tableQ * ix->totalBins, st);
-                  touched.alloc((size_t)tableQ * std::max(nG, 1), st);
-                  if (wantFrags) BANI_CUDA(cudaMemsetAsync(table64.p, 0, table64.bytes(), st));
-                  else BANI_CUDA(cudaMemsetAsync(table.p, 0, table.bytes(), st));
-                  BANI_CUDA(cudaMemsetAsync(touched.p, 0, touched.bytes(), st));
-                }
-                CgiArgs ca; ca.rows = rows.p; ca.rFrag = rFrag.p; ca.R = R; ca.fragQuery = d_fragQuery.p;
-                ca.contigGenome = ix->contigGenome.p; ca.contigBinOff = ix->contigBinOff.p; ca.fragLen = fragLen;
-                ca.totalBins = ix->totalBins; ca.nGenomes = nG; ca.table = table.p; ca.touched = touched.p;
-                BANI_SCRATCH(int32_t, oCount, (size_t)nQc * nG);
-                DevBuf<float> oIdent((size_t)nQc * nG, st);
-                if (!wantFrags) {
-                  Stage sg(ctx, "cgi", 48.0 * R);
-                  for (int qa = 0; qa < nQc; qa += (int)tableQ) {
-                    const int nPass = std::min<int>((int)tableQ, nQc - qa);
-                    ca.qLo = qa; ca.qHi = qa + nPass;
-                    cgi_scatter_kernel<<<nblk(R), 256, 0, st>>>(ca);
-                    ctx->launches++; pp[P_CGI_PASSES]++;
-                    cgi_sum_kernel<<<nblk((uint64_t)nPass * nG), 256, 0, st>>>(table.p, touched.p, ix->contigBinOff.p, d_gce.p,
-                                                                             ix->totalBins, nG, nPass, oCount.p + (size_t)qa * nG, oIdent.p + (size_t)qa * nG);
-                    ctx->launches++;
-                  }
-                } else {
-                  // fragment-row mode: scatter 64-bit keys, emit each bin's winning row before the sum clears the bin, then
-                  // sort the piece's winners by (query slot, global bin) -- unique keys, so the order is deterministic
-                  BANI_SCRATCH(uint8_t, win, R);
-                  BANI_SCRATCH(unsigned long long, emKey, R);
-                  BANI_SCRATCH(unsigned long long, emKeySorted, R);
-                  BANI_SCRATCH(uint32_t, emRow, R);
-                  BANI_SCRATCH(uint32_t, emRowSorted, R);
-                  BANI_SCRATCH(uint32_t, emCount, 1);
-                  BANI_CUDA(cudaMemsetAsync(emCount.p, 0, 4, st));
-                  CgiFragArgs fa; fa.table = table64.p; fa.win = win.p; fa.key = emKey.p; fa.row = emRow.p; fa.count = emCount.p;
-                  Stage sg(ctx, "cgi_frags", 64.0 * R);
-                  for (int qa = 0; qa < nQc; qa += (int)tableQ) {
-                    const int nPass = std::min<int>((int)tableQ, nQc - qa);
-                    ca.qLo = qa; ca.qHi = qa + nPass;
-                    cgi_scatter_frag_kernel<<<nblk(R), 256, 0, st>>>(ca, fa);
-                    ctx->launches++; pp[P_CGI_PASSES]++;
-                    cgi_emit_kernel<<<nblk(R), 256, 0, st>>>(ca, fa);
-                    ctx->launches++;
-                    cgi_sum_frag_kernel<<<nblk((uint64_t)nPass * nG), 256, 0, st>>>(table64.p, touched.p, ix->contigBinOff.p, d_gce.p,
-                                                                                  ix->totalBins, nG, nPass, oCount.p + (size_t)qa * nG, oIdent.p + (size_t)qa * nG);
-                    ctx->launches++;
-                  }
-                  uint32_t nEm = 0;
-                  BANI_CUDA(cudaMemcpyAsync(&nEm, emCount.p, 4, cudaMemcpyDeviceToHost, st));
-                  BANI_CUDA(cudaStreamSynchronize(st));
-                  if (nEm > 0) {
-                    int qBits = 0; while ((1 << qBits) < nQc) qBits++;
-                    { size_t tb = cub_sort_pairs_u64_u32_temp(nEm);
-                      BANI_SCRATCH(uint8_t, tmp, tb);
-                      cub_sort_pairs_u64_u32(tmp.p, tb, (const uint64_t *)emKey.p, (uint64_t *)emKeySorted.p, emRow.p, emRowSorted.p, nEm, 32 + qBits, st); }
-                    BANI_SCRATCH(bani_frag_mapping, dFrags, nEm);
-                    cgi_frag_gather_kernel<<<nblk(nEm), 256, 0, st>>>(rows.p, emKeySorted.p, emRowSorted.p, nEm, dFrags.p);
-                    ctx->launches++;
-                    hFrags.resize(nEm);
-                    BANI_CUDA(cudaMemcpyAsync(hFrags.data(), dFrags.p, sizeof(bani_frag_mapping) * (size_t)nEm, cudaMemcpyDeviceToHost, st));
-                  }
-                }
-                ctx->mark("piece: cgi launched");
-                BANI_CUDA(cudaMemcpyAsync(hCount.data(), oCount.p, 4 * (size_t)nQc * nG, cudaMemcpyDeviceToHost, st));
-                BANI_CUDA(cudaMemcpyAsync(hIdent.data(), oIdent.p, 4 * (size_t)nQc * nG, cudaMemcpyDeviceToHost, st));
-                BANI_CUDA(cudaStreamSynchronize(st));
-                ctx->mark("piece: identity tables on host");
-              }
-            }
-          }
-        }
+    const QSketch *qs = sketches[si];
+    if (!qs) fail(BANI_ERR_ARG, "null query sketch");
+    if (qs->device != ctx->device) fail(BANI_ERR_ARG, "query sketch lives on another device");
+    if (qs->k != k || qs->w != w || qs->fragLen != fragLen) fail(BANI_ERR_ARG, "query sketch was built with other parameters");
+    std::deque<const QPiece *> work;
+    std::vector<std::unique_ptr<QPiece>> slices;
+    for (const auto &pcp : qs->pieces) work.push_back(pcp.get());
+    while (!work.empty()) {
+      const QPiece &pc = *work.front();
+      work.pop_front();
+      const PathId r = map_piece(ctx, ix, *qs, pc, cgi.get(), wantRows, out);
+      if (r != P_PIECE_MAPPED) {
+        // halve the piece at a query boundary (by fragments) and do the halves instead
+        if (ctx->flags.countPaths) ctx->paths[r]++;
+        int qm = 1;
+        while (qm < pc.nq - 1 && pc.qFragOff[qm] < pc.F / 2) qm++;
+        slices.push_back(slice_piece(ctx, pc, qm, pc.nq)); work.push_front(slices.back().get());
+        slices.push_back(slice_piece(ctx, pc, 0, qm)); work.push_front(slices.back().get());
       }
-    piece_done:
-      BANI_CUDA(cudaGetLastError());
-      BANI_CUDA(cudaStreamSynchronize(st));
-    }
-    if (!split) { out.ctr.fragments += F; out.ctr.sum_s += (F > 0 && ix->M > 0) ? T : 0; }
-    if (!split && countPaths) {
-      pp[P_PIECE_MAPPED]++;
-      for (int i = 0; i < NPATH; i++) ctx->paths[i] += pp[i];
-    }
-    if (wantCgi && !split && !hCount.empty()) {
-      append_cgi_rows(hCount.data(), hIdent.data(), nQc, nG, qs->queryId.data() + q0, qs->totalFragments.data() + q0, out.cgi);
-    }
-    if (wantCgi && !split) {
-      for (bani_cgi_result r : hPairs) {
-        if (r.countSeq <= 0) continue;
-        const int slot = r.qryGenomeId;
-        r.qryGenomeId = qs->queryId[q0 + slot]; r.totalQueryFragments = (int32_t)qs->totalFragments[q0 + slot];
-        out.cgi.push_back(r);
+      if (pc.F > 0 && ix->M > 0) {
+        BANI_CUDA(cudaGetLastError());
+        BANI_CUDA(cudaStreamSynchronize(st));        // the piece's scratch is reused by the next one
       }
+      ctx->mark("piece: rows assembled");
     }
-    if (wantFrags && !split) {
-      for (auto &m : hFrags) m.qryGenomeId = qs->queryId[q0 + m.qryGenomeId];
-      out.frags.insert(out.frags.end(), hFrags.begin(), hFrags.end());
-    }
-    ctx->mark("piece: rows assembled");
-   }
   }
   ctx->mark("qsketch_map: pieces done");
 }
